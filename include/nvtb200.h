@@ -353,7 +353,10 @@ int nvtb_encode_apply(const nvtb_vocab_t* v, const nvtb_col_t* key_host,
  * column j of the matrix, out[j][i] = stats[row(key_i)][j] cast to
  * out_dtypes[j] (I32|I64|F32|F64), or miss_vals[j] (NaN == null; the global
  * mean for TargetEncoding, target_encoding.py:378-380) when the key is
- * absent. */
+ * absent.  valid_out (NULL, or one entry per output column, each NULL or a
+ * device bitmask of ceil(n / 32) 4-byte-aligned words): bit i set (Arrow
+ * layout, LSB first) when key i has a row and that value is not NaN.  An
+ * integer output holds 0 where the bit is clear. */
 typedef struct nvtb_groupstats nvtb_groupstats_t;
 /* null_row: row of `stats` that null keys join to (pandas/cuDF merge matches
  * null with null, and dropna=False makes the null key a group), or -1. */
@@ -366,7 +369,7 @@ int nvtb_groupstats_gather(const nvtb_groupstats_t* g,
                            const int* cols_host, int ncols_out,
                            const double* miss_vals_host,
                            void* const* out_host, const int* out_dtypes_host,
-                           void* stream);
+                           uint8_t* const* valid_out_host, void* stream);
 
 /* ---- cross-GPU collectives of the fit path (SURVEY.md 8e) ---------------------------------
  * nvtb_comm_t wraps an ncclComm_t: created here (rank 0 makes a unique id, the host runtime

@@ -93,7 +93,7 @@ _SIGNATURES = {
     "nvtb_infer_fill_host": (c_int, [c_void_p, c_int, c_int64, c_double]),
     "nvtb_groupstats_create": (c_int, [POINTER(c_void_p), c_void_p, c_int64, c_void_p, c_int, c_int64, c_void_p]),
     "nvtb_groupstats_destroy": (c_int, [c_void_p]),
-    "nvtb_groupstats_gather": (c_int, [c_void_p, POINTER(nvtb_col_t), c_int64, POINTER(c_int), c_int, POINTER(c_double), POINTER(c_void_p), POINTER(c_int), c_void_p]),
+    "nvtb_groupstats_gather": (c_int, [c_void_p, POINTER(nvtb_col_t), c_int64, POINTER(c_int), c_int, POINTER(c_double), POINTER(c_void_p), POINTER(c_int), POINTER(c_void_p), c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -405,27 +405,42 @@ encode_smem_kernel(const int32_t* __restrict__ keys, const uint8_t* __restrict__
 constexpr int kMaxGatherCols = 16;
 struct GatherOut {
   void* out[kMaxGatherCols];
+  uint32_t* valid[kMaxGatherCols];   // optional validity bitmask of out[j], or nullptr
   double miss[kMaxGatherCols];
   int32_t col[kMaxGatherCols];
   int32_t dtype[kMaxGatherCols];
   int32_t ncols;
 };
 
+// A row of out[j] is valid when its key has a row in the matrix and that value is not NaN.  An
+// integer output holds 0 where it is not valid, so the bitmask is what tells a missing statistic
+// from a real 0.  A warp covers 32 consecutive rows (blockDim and the grid stride are multiples
+// of 32), so one ballot gives one 32-bit word of the LSB-first bitmask.
 template <typename KeyT>
 __global__ void __launch_bounds__(kThreads)
 gather_stats_kernel(const KeyT* __restrict__ keys, const uint8_t* __restrict__ mask,
                     int64_t n, Lookup t, int64_t null_row,
                     const double* __restrict__ stats, int width, GatherOut go) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const int64_t row = valid1(mask, i) ? lookup_find(t, (int64_t)keys[i]) : null_row;
+  const int lane = threadIdx.x & 31;
+  // whole warps iterate together (the ballot below needs every lane)
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i - lane < n; i += stride) {
+    const bool in = i < n;
+    const int64_t row = !in ? -1 : valid1(mask, i) ? lookup_find(t, (int64_t)keys[i]) : null_row;
     for (int j = 0; j < go.ncols; ++j) {
       const double v = row >= 0 ? __ldg(stats + row * width + go.col[j]) : go.miss[j];
-      switch (go.dtype[j]) {
-        case NVTB_I32: ((int32_t*)go.out[j])[i] = (int32_t)v; break;
-        case NVTB_I64: ((int64_t*)go.out[j])[i] = (int64_t)v; break;
-        case NVTB_F32: ((float*)go.out[j])[i] = (float)v; break;
-        default:       ((double*)go.out[j])[i] = v; break;
+      const bool ok = row >= 0 && v == v;
+      if (in) {
+        switch (go.dtype[j]) {
+          case NVTB_I32: ((int32_t*)go.out[j])[i] = v == v ? (int32_t)v : 0; break;
+          case NVTB_I64: ((int64_t*)go.out[j])[i] = v == v ? (int64_t)v : 0; break;
+          case NVTB_F32: ((float*)go.out[j])[i] = (float)v; break;
+          default:       ((double*)go.out[j])[i] = v; break;
+        }
+      }
+      if (go.valid[j] != nullptr) {
+        const unsigned bits = __ballot_sync(0xFFFFFFFFu, in && ok);
+        if (lane == 0) go.valid[j][i >> 5] = bits;
       }
     }
   }
@@ -1420,7 +1435,8 @@ int nvtb_groupstats_destroy(nvtb_groupstats_t* g) {
 
 int nvtb_groupstats_gather(const nvtb_groupstats_t* g, const nvtb_col_t* key, int64_t n,
                            const int* cols, int ncols_out, const double* miss_vals,
-                           void* const* out, const int* out_dtypes, void* stream) {
+                           void* const* out, const int* out_dtypes, uint8_t* const* valid_out,
+                           void* stream) {
   NVTB_REQUIRE(g != nullptr && key != nullptr && n >= 0, "NULL argument or n < 0");
   NVTB_REQUIRE(key->dtype == NVTB_I32 || key->dtype == NVTB_I64, "key dtype must be int32 or int64");
   NVTB_REQUIRE(ncols_out >= 1 && ncols_out <= kMaxGatherCols, "ncols_out must be in [1, 16]");
@@ -1435,6 +1451,8 @@ int nvtb_groupstats_gather(const nvtb_groupstats_t* g, const nvtb_col_t* key, in
     NVTB_REQUIRE(out[j] != nullptr, "out column is NULL");
     NVTB_REQUIRE(out_dtypes[j] >= NVTB_I32 && out_dtypes[j] <= NVTB_F64, "bad out dtype");
     go.out[j] = out[j]; go.miss[j] = miss_vals[j]; go.col[j] = cols[j]; go.dtype[j] = out_dtypes[j];
+    go.valid[j] = valid_out != nullptr ? reinterpret_cast<uint32_t*>(valid_out[j]) : nullptr;
+    NVTB_REQUIRE((reinterpret_cast<uintptr_t>(go.valid[j]) & 3u) == 0, "validity output must be 4-byte aligned");
   }
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = (int)std::min<int64_t>((n + kThreads - 1) / kThreads, (int64_t)sm_count() * 8);

@@ -566,12 +566,29 @@ class GroupStats:
         except Exception:
             pass
 
+    MAX_COLS = 16   # output columns of one nvtb_groupstats_gather launch (kMaxGatherCols, csrc/vocab.cu)
+
     def gather(self, key: Column, cols: Sequence[int], miss_vals: Sequence[float], out_dtypes) -> List[torch.Tensor]:
+        """one output tensor per entry of `cols`; more than MAX_COLS take several launches"""
+        return [c.data for c in self.gather_columns(key, cols, miss_vals, out_dtypes)]
+
+    def gather_columns(self, key: Column, cols: Sequence[int], miss_vals: Sequence[float], out_dtypes,
+                       masked: Sequence[bool] = ()) -> List[Column]:
+        """as gather(), as Columns; output j with masked[j] gets a validity bitmask that is clear
+        where the key has no row or the statistic is NaN (an integer output holds 0 there)"""
         n = key.data.numel()
+        dev = key.data.device
         codes = [dtype_code(d) for d in out_dtypes]
-        outs = [torch.empty(n, dtype=_CODE2TORCH[c], device=key.data.device) for c in codes]
-        _lib.check(self.lib.nvtb_groupstats_gather(
-            self.h, _descs([key]), n, _lib.int_array(cols), len(cols), _lib.double_array(miss_vals),
-            _lib.ptr_array([o.data_ptr() for o in outs]), _lib.int_array(codes), _lib.stream_ptr()))
-        _count()
-        return outs
+        outs = [torch.empty(n, dtype=_CODE2TORCH[c], device=dev) for c in codes]
+        nbytes = (((n + 7) // 8 + 31) // 32) * 32          # pack_validity's padding (>= ceil(n/32) words)
+        valid = [torch.zeros(nbytes, dtype=torch.uint8, device=dev) if j < len(masked) and masked[j] else None
+                 for j in range(len(cols))]
+        for s in range(0, len(cols), self.MAX_COLS):
+            e = s + self.MAX_COLS
+            vptrs = [v.data_ptr() if v is not None else None for v in valid[s:e]]
+            _lib.check(self.lib.nvtb_groupstats_gather(
+                self.h, _descs([key]), n, _lib.int_array(cols[s:e]), len(cols[s:e]), _lib.double_array(miss_vals[s:e]),
+                _lib.ptr_array([o.data_ptr() for o in outs[s:e]]), _lib.int_array(codes[s:e]),
+                _lib.ptr_array(vptrs) if any(vptrs) else None, _lib.stream_ptr()))
+            _count()
+        return [Column(o, v) for o, v in zip(outs, valid)]

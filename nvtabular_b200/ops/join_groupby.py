@@ -20,6 +20,24 @@ from .base import StatOperator
 from .keyspace import ComboKeySpace, KeySpace, _leaf
 
 AGG_DTYPES = {"count": np.int32, "std": np.float32, "var": np.float32, "mean": np.float32}  # join_groupby.py:29-34
+# sum / min / max keep the dtype the statistics file holds instead of float64 (only AGG_DTYPES are
+# recast, join_groupby.py:211-214, 252-261): pandas / cuDF reduce a float32 column in float32, keep
+# min / max of an int column in its dtype, and sum an int column into int64 (pandas keeps int32 for
+# an int32 sum that fits, and widens one that does not).  The engine sums in fp64: an int64 sum is
+# exact while |sum| < 2^53.
+_TYPED_STATS = ("sum", "min", "max")
+_KEEP_DTYPES = (np.dtype(np.float32), np.dtype(np.int32), np.dtype(np.int64))
+
+
+def _kept_dtype(dt, stat="min"):
+    """the dtype of statistic `stat` (sum/min/max) of a column of dtype `dt`, or None (float64)"""
+    try:
+        dt = np.dtype(getattr(dt, "numpy_dtype", dt)) if dt is not None else None
+    except TypeError:
+        return None
+    if dt not in _KEEP_DTYPES:
+        return None
+    return np.dtype(np.int64) if stat == "sum" and dt.kind == "i" else dt
 
 
 def _make_name(*args, sep="_"):
@@ -51,7 +69,8 @@ class GroupTable:
         stat_names = [c for c in df.columns if c.startswith(name + sep)]
         key_names = [c for c in df.columns if c not in stat_names]
         space, keys, isnull = keys_from_frame(df, key_names)
-        mat = torch.from_numpy(df[stat_names].to_numpy(dtype=np.float64)).to(keys.device) if stat_names else \
+        mat = torch.from_numpy(df[stat_names].to_numpy(dtype=np.float64, na_value=np.nan)).to(keys.device) \
+            if stat_names else \
             torch.zeros((len(df), 1), dtype=torch.float64, device=keys.device)
         null_idx = torch.nonzero(isnull).flatten()
         keep = ~isnull
@@ -61,7 +80,8 @@ class GroupTable:
             stats = torch.cat([stats, mat[null_idx[:1]]], dim=0)
             null_row = int(keep.sum().item())
         t = cls(name, key_names, space, keys[keep].contiguous(), stat_names, stats.contiguous(), null_row, None)
-        t.f32_stats = {c for c in stat_names if df[c].dtype == np.float32 and c.rsplit(sep, 1)[-1] in ("sum", "min", "max")}
+        t.stat_dtypes = {c: _kept_dtype(df[c].dtype) for c in stat_names
+                         if c.rsplit(sep, 1)[-1] in _TYPED_STATS and _kept_dtype(df[c].dtype) is not None}
         t.path = path
         return t
 
@@ -71,13 +91,16 @@ class GroupTable:
         st = self.stats.cpu().numpy()
         data = key_columns(self.space, self.key_names, k, with_null_row=self.null_row >= 0)
         rows = len(k) + (1 if self.null_row >= 0 else 0)
-        f32 = getattr(self, "f32_stats", ())
+        typed = getattr(self, "stat_dtypes", {})
         for j, sn in enumerate(self.stat_names):
             col = st[:rows, j]
             if sn.endswith("_count"):                  # the reference's file holds integer counts
                 col = col.astype(np.int64)
-            elif sn in f32:                            # ... and float32 sums of float32 columns
-                col = col.astype(np.float32)
+            elif sn in typed and (typed[sn].kind == "f" or not np.isnan(col).any()):
+                col = col.astype(typed[sn])            # ... and sum/min/max in the column's dtype
+            elif sn in typed:                          # an int min/max of a group without values
+                col = pd.array(np.where(np.isnan(col), 0, col).astype(typed[sn]), dtype=f"Int{typed[sn].itemsize * 8}")
+                col[np.isnan(st[:rows, j])] = pd.NA
             data[sn] = col
         return pd.DataFrame(data)
 
@@ -235,16 +258,20 @@ class JoinGroupby(StatOperator):
             for j, sn in enumerate(t.stat_names):
                 if sn in new_df:
                     continue
-                dt = np.float32 if sn in getattr(t, "f32_stats", ()) else np.float64
+                dt = getattr(t, "stat_dtypes", {}).get(sn, np.float64)
                 for agg, d in AGG_DTYPES.items():
                     if sn.endswith(f"{self.name_sep}{agg}"):
                         dt = d
                 idx.append(j); dts.append(dt); out_names.append(sn)
             if not idx:
                 continue
-            outs = t.handle.gather(key, idx, [float("nan")] * len(idx), dts)
+            # an integer output is null where the key has no group (a key the fit never saw, or a null
+            # key when the fit had none) or the statistic is NaN: the reference's left merge leaves
+            # those rows missing, it must not read as 0
+            masked = [np.dtype(d).kind != "f" for d in dts]
+            outs = t.handle.gather_columns(key, idx, [float("nan")] * len(idx), dts, masked)
             for sn, o in zip(out_names, outs):
-                new_df[sn] = Column(o)
+                new_df[sn] = o
         return new_df
 
     def _table(self, name) -> GroupTable:
@@ -282,6 +309,10 @@ class JoinGroupby(StatOperator):
             if new_schema.name.endswith(f"{self.name_sep}{agg}"):
                 dtype = d
                 break
+        else:   # sum / min / max: from the dtype of the continuous column (the first source)
+            stat = new_schema.name.rsplit(self.name_sep, 1)[-1]
+            if stat in _TYPED_STATS:
+                dtype = _kept_dtype(new_schema.dtype, stat) or dtype
         return new_schema.with_dtype(dtype, False, False)
 
     def export_tables(self, new_path) -> Dict[str, str]:
@@ -320,9 +351,14 @@ def fit_group_table(name, names, parts, cont, stats, sep="_") -> GroupTable:
         key = space.keys_for([df[n] for n in names]) if len(names) > 1 else space.keys_for(df[names[0]])
         agg.insert(key, [_leaf(df[c]) for c in cont])
     t = build_group_table(name, names, space, agg, cont, stats, sep)
-    # pandas / cuDF keep sum, min and max of a float32 column in float32 (the stat file of
-    # the reference holds that dtype, join_groupby.py:200-215 reads it back unchanged)
-    import torch as _torch
-    t.f32_stats = {_make_name(name, c, a, sep=sep) for c in cont for a in ("sum", "min", "max")
-                   if parts and _leaf(parts[0][c]).data.dtype == _torch.float32}
+    # sum / min / max in the dtype the reference's stat file holds (see _kept_dtype; join_groupby.py
+    # :200-215 reads it back unchanged), decided by the column's dtype alone so that it matches the
+    # output schema.  Rows without a value are nulls of the integer outputs (transform).
+    t.stat_dtypes = {}
+    for c in cont:
+        src = str(_leaf(parts[0][c]).data.dtype).replace("torch.", "") if parts else None
+        for a in _TYPED_STATS:
+            dt = _kept_dtype(src, a)
+            if dt is not None:
+                t.stat_dtypes[_make_name(name, c, a, sep=sep)] = dt
     return t

@@ -70,6 +70,48 @@ def test_movielens_shape_joingroupby_targetencoding_vs_oracle(nvt, ops, tmp_path
         np.testing.assert_allclose(out[c].to_numpy(), exp_t[c].to_numpy(), rtol=2e-6, err_msg=c)
 
 
+# One 5e6-row partition: with no hint and no estimate the operator's first insert is the blind
+# 2^20-row sample (4 M-slot table), from which ~2e6 keys are estimated, and prepare() then grows
+# the table before the rest of the rows: the payload goes through rehash_kernel.  TargetEncoding's
+# packed (fold, group) keys are int64, so the wide table with payload grows the same way.
+def test_groupby_stats_through_table_growth_vs_oracle(nvt, ops, tmp_path):
+    rows = 5_000_000
+    rng = np.random.default_rng(12)
+    x = rng.normal(3.0, 2.0, rows)
+    x[rng.random(rows) < 0.05] = np.nan
+    df = pd.DataFrame({
+        "g": ((rng.integers(0, 2_000_000, rows) * 2654435761) % (1 << 31)).astype(np.int32),
+        "h": rng.integers(0, 4, rows).astype(np.int32),
+        "x": x,                                                           # float64 with NaN
+        "i": rng.integers(-1000, 1000, rows).astype(np.int32),            # int32, no nulls
+        "f": (rng.integers(1, 11, rows) * 0.5).astype(np.float32)})      # float32
+    groups = ["g", ["g", "h"]]
+    stats = ["count", "sum", "mean", "std", "var", "min", "max"]
+    jg = groups >> ops.JoinGroupby(out_path=str(tmp_path), cont_cols=["x", "i", "f"], stats=stats)
+    te = groups >> ops.TargetEncoding(["f", "i"], kfold=3, p_smooth=20, out_path=str(tmp_path))
+    wf = nvt.Workflow(jg + te)
+    out = wf.fit_transform(nvt.Dataset(df, npartitions=1)).to_ddf().compute()
+
+    tabs = {"g": groupby_stats([df], ["g"], ["x", "i", "f"], stats),
+            "g_h": groupby_stats([df], ["g", "h"], ["x", "i", "f"], stats)}
+    exp_j = join_groupby_transform(df, groups, tabs)
+    assert sorted(c for c in out.columns if not c.startswith("TE_")) == sorted(exp_j.columns)
+    for c in exp_j.columns:
+        # the sum of an int column is int64 (exact); pandas keeps int32 for an int32 sum that fits
+        want = np.dtype("int64") if c.endswith("_i_sum") else exp_j[c].dtype
+        assert out[c].dtype == want, (c, out[c].dtype, exp_j[c].dtype)
+        if c.endswith("count") or np.issubdtype(exp_j[c].dtype, np.integer):
+            np.testing.assert_array_equal(out[c].to_numpy(), exp_j[c].to_numpy(), err_msg=c)
+        else:
+            np.testing.assert_allclose(out[c].to_numpy(), exp_j[c].to_numpy(), rtol=2e-5, atol=1e-5,
+                                       equal_nan=True, err_msg=c)
+    exp_t = pd.concat(target_encoding([df], groups, ["f", "i"], kfold=3, p_smooth=20)[0], ignore_index=True)
+    assert sorted(c for c in out.columns if c.startswith("TE_")) == sorted(exp_t.columns)
+    for c in exp_t.columns:
+        assert out[c].dtype == exp_t[c].dtype == np.float32, c
+        np.testing.assert_allclose(out[c].to_numpy(), exp_t[c].to_numpy(), rtol=2e-6, err_msg=c)
+
+
 # TargetEncoding, random frame, every fold count the reference's tests use
 @pytest.mark.parametrize("kfold", [1, 3, 5])
 @pytest.mark.parametrize("npartitions", [1, 3])

@@ -436,6 +436,54 @@ def test_joingroupby_random_vs_oracle(nvt, ops, tmp_path):
             np.testing.assert_array_equal(out[c].to_numpy(), exp[c].to_numpy())
 
 
+def test_joingroupby_int_columns_on_unseen_and_null_keys_vs_oracle(nvt, ops, tmp_path):
+    """Fit on one frame, transform it and a second frame whose keys the fit never saw, with null
+    keys the fit had no group for.  Integer statistics: sum int64 (exact beyond 2^31, where an
+    int32 sum would overflow), min/max in the column's dtype, and missing where the reference's
+    left merge finds no group, never 0."""
+    rng = np.random.default_rng(19)
+    n = 30_000
+    train = pd.DataFrame({"u": rng.integers(0, 300, n).astype("int32"), "m": rng.integers(0, 20, n).astype("int32"),
+                          "big": rng.integers(1 << 29, (1 << 31) - 1, n).astype("int32"),   # group sums > 2^31
+                          "small": rng.integers(-50, 50, n).astype("int32"),
+                          "w": rng.integers(-(1 << 40), 1 << 40, n).astype("int64"),
+                          "r": rng.normal(0, 1, n)})
+    m = 4000
+    test = pd.DataFrame({"u": pd.array(rng.integers(0, 400, m), dtype="Int32"),     # 1/4 unseen keys
+                         "m": rng.integers(0, 25, m).astype("int32")})
+    test.loc[rng.random(m) < 0.05, "u"] = pd.NA                                     # no null group in the fit
+    for c in ("big", "small", "w", "r"):
+        test[c] = train[c].iloc[:m].to_numpy()
+    conts, groups = ["big", "small", "w", "r"], ["u", ["u", "m"]]
+    stats = ["sum", "min", "max", "mean"]    # "count" of a missing key cannot be cast to int32 by the reference
+    wf = nvt.Workflow(groups >> ops.JoinGroupby(out_path=str(tmp_path), stats=stats, cont_cols=conts))
+    wf.fit(nvt.Dataset(train))
+    tabs = {"u": groupby_stats(train, ["u"], conts, stats), "u_m": groupby_stats(train, ["u", "m"], conts, stats)}
+    assert tabs["u"]["u_big_sum"].max() > (1 << 31)
+    schema = {c: np.dtype(wf.output_schema[c].dtype) for c in wf.output_schema.column_names}
+    for frame, unseen in ((train, False), (test, True)):
+        out = wf.transform(nvt.Dataset(frame)).to_ddf().compute()
+        exp = join_groupby_transform(frame, groups, tabs)
+        assert sorted(out.columns) == sorted(exp.columns)
+        for c in exp.columns:
+            stat, src = c.rsplit("_", 1)[-1], c.split("_")[-2]
+            want = np.dtype("int64") if stat == "sum" and src != "r" else schema[c]
+            if not unseen:
+                # pandas keeps int32 for an int32 sum that fits; the engine always sums ints into int64
+                assert schema[c] == want and out[c].dtype == want, (c, out[c].dtype, want)
+            else:
+                # rows without a group: missing, so pandas and the engine both hold float64 NaN
+                assert out[c].dtype == exp[c].dtype, (c, out[c].dtype, exp[c].dtype)
+                if np.dtype(schema[c]).kind == "i":
+                    assert out[c].isna().to_numpy().sum() > m // 5, c
+            if c.endswith("_mean") or src == "r":
+                np.testing.assert_allclose(out[c].to_numpy(dtype=np.float64), exp[c].to_numpy(dtype=np.float64),
+                                           rtol=1e-6, equal_nan=True, err_msg=c)
+            else:
+                np.testing.assert_array_equal(out[c].to_numpy(dtype=np.float64), exp[c].to_numpy(dtype=np.float64),
+                                              err_msg=c)
+
+
 # reference tests/unit/ops/test_target_encode.py:38-84, 111-147
 @pytest.mark.parametrize("kfold", [1, 3])
 @pytest.mark.parametrize("npartitions", [1, 2])
