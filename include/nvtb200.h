@@ -371,6 +371,89 @@ int nvtb_groupstats_gather(const nvtb_groupstats_t* g,
                            void* const* out_host, const int* out_dtypes_host,
                            uint8_t* const* valid_out_host, void* stream);
 
+/* ---- session group-by: Groupby operator and Dataset.shuffle_by_keys (csrc/groupby.cu, K8) ----
+ * Per partition, replaces the cuDF / pandas calls of reference nvtabular/ops/groupby.py:
+ * df.sort_values(sort_cols, ascending) (groupby.py:118-120), df.groupby(groupby_cols).agg(...)
+ * (groupby.py:222-227) and _first_or_last's list.get(0) / list.get(-1) (groupby.py:290-313).
+ *
+ * nvtb_gb_order_codes: one pass over a column -> codes_out[i], a uint64 whose unsigned order is
+ * the column's order (int: sign bit flipped; float: order-preserving image with -0.0 made +0.0;
+ * uint8: the value; a string column passes its int32 dictionary codes), valid_out (bitmask,
+ * ceil(n/8) bytes: clear for a null or NaN row), and stats_dev[3] = {min, max, n_valid} of the
+ * valid codes.  key_valid (may be NULL) receives the bitmask too, ANDed into it when
+ * and_key_valid != 0 (the "every key is valid" mask of a multi-column key).  codes_out 32-byte
+ * aligned. */
+int nvtb_gb_order_codes(const nvtb_col_t* col, int64_t n, uint64_t* codes_out, uint8_t* valid_out,
+                        uint8_t* key_valid, int and_key_valid, uint64_t* stats_dev, void* stream);
+/* One chunk of one field of a row-ordering round.  A field's value for a row:
+ *   mode 0  codes[row] - min                          (a group key; null-key rows are flagged)
+ *   mode 1  valid ? codes[row] - min : span + 1        (ascending, nulls last)
+ *   mode 2  valid ? span - (codes[row] - min) : span + 1  (descending, nulls last)
+ *   mode 3  valid ? 0 : 1                              (a null flag)
+ * and the chunk takes bits [lo, lo + nbits) of it. */
+typedef struct {
+  const uint64_t* codes;
+  const uint8_t* valid;
+  uint64_t min;
+  uint64_t span;
+  int32_t mode;
+  int32_t lo;
+  int32_t nbits;
+  int32_t _pad;
+} nvtb_gb_chunk_t;
+/* Order rows 0..n-1 by fields F1 > F2 > ...: elements (packed fields << row_bits) | row are
+ * sorted by LSD rounds; round k packs round_sizes_host[k] consecutive chunks of chunks_host
+ * (least significant first, at most 64 - row_bits bits) and sorts those bits with the stable
+ * radix primitive (radix.cuh).  Later rounds rewrite the high bits in place from the row, so
+ * stability carries the earlier rounds.  The round plan comes from the host
+ * (nvtabular_b200/ops/groupby.py plan_rounds).  No rounds: elements are the rows in order.
+ * The result ends in elems (*result_in_tmp_host = 0) or tmp (1).  n < 2^32. */
+int nvtb_gb_order_rows(const nvtb_gb_chunk_t* chunks_host, const int* round_sizes_host, int n_rounds,
+                       int64_t n, int row_bits, uint64_t* elems, uint64_t* tmp,
+                       int* result_in_tmp_host, void* stream);
+/* Segments of the ordered rows: a position starts a group when its row's keys are all valid
+ * (key_valid, NULL = all) and one of the n_keys key codes differs from the previous position's.
+ * flags: ceil(n/8) bytes; tile_scan: ceil(n/2048) uint32.  counts_host = {groups, rows with valid
+ * keys}.  Synchronises.  nvtb_gb_segments_write then writes off_out[groups + 1] (int64). */
+int nvtb_gb_segments_count(const uint64_t* order, int64_t n, int row_bits,
+                           const uint64_t* const* key_codes_host, int n_keys,
+                           const uint8_t* key_valid, uint8_t* flags, uint32_t* tile_scan,
+                           int64_t* counts_host, void* stream);
+int nvtb_gb_segments_write(const uint8_t* flags, const uint32_t* tile_scan, int64_t n,
+                           int64_t n_groups, int64_t n_kept, int64_t* off_out, void* stream);
+/* gid_out[p] = g for off[g] <= p < off[g + 1], p < n */
+int nvtb_gb_segment_ids(const int64_t* off, int64_t n_groups, int64_t n, uint64_t* gid_out,
+                        void* stream);
+/* Gather data + validity: which 0: out[i] = col[row(i)] (i < m); 1: out[g] = col[row(off[g])];
+ * 2: out[g] = col[row(off[g + 1] - 1)]; row(p) = order ? order[p] & row_mask : p.  which | 4:
+ * the column is a float key, -0.0 is written as +0.0.  out_valid (may be NULL) receives
+ * ceil(m/8) bitmask bytes. */
+int nvtb_gb_gather(const nvtb_col_t* col, const uint64_t* order, uint64_t row_mask,
+                   const int64_t* off, int64_t m, int which, void* out, uint8_t* out_valid,
+                   void* stream);
+/* Per segment [off[g], off[g+1]) of a column in group order, over its valid non-NaN values, in
+ * fp64 and a fixed order: outs_host[7] = {count int32, sum f32, mean f32, var f32, std f32
+ * (ddof 1, two passes), min, max (the column's dtype)}; NULL entries are skipped.  sum of no
+ * values is 0; mean / min / max of none are NaN; var / std of fewer than 2 are NaN.  valid_host
+ * (NULL or 2 zeroed bitmasks, 4-byte aligned): bit g set when the integer min / max of g exists. */
+int nvtb_gb_reduce(const nvtb_col_t* col, const int64_t* off, int64_t n_groups,
+                   void* const* outs_host, uint8_t* const* valid_host, void* stream);
+/* median (f32; the fp64 mean of the two middle values at an even count) and nunique (int32) per
+ * segment, from positions `order` sorted by (group, value code) with null values last in a group
+ * (nvtb_gb_order_rows), codes / codes_valid from nvtb_gb_order_codes of col.  Either output may
+ * be NULL. */
+int nvtb_gb_rank_stats(const nvtb_col_t* col, const uint64_t* codes, const uint8_t* codes_valid,
+                       const uint64_t* order, uint64_t row_mask, const int64_t* off,
+                       int64_t n_groups, float* median_out, int32_t* nunique_out, void* stream);
+
+/* Sub-lists [lo[g], hi[g]) of a list column's leaves, concatenated (first / last of a list input
+ * column, reference test_groupby_list_first_last).  Called twice: with out == NULL it writes
+ * off_out[m + 1] and *total_host (synchronises); then with out (total_host leaves of the leaf
+ * dtype) and out_valid (NULL, or a zeroed 4-byte-aligned bitmask) it copies the leaves. */
+int nvtb_gb_list_rows(const nvtb_col_t* leaves, const int64_t* lo, const int64_t* hi, int64_t m,
+                      int64_t* off_out, void* out, uint8_t* out_valid, int64_t* total_host,
+                      void* stream);
+
 /* ---- cross-GPU collectives of the fit path (SURVEY.md 8e) ---------------------------------
  * nvtb_comm_t wraps an ncclComm_t: created here (rank 0 makes a unique id, the host runtime
  * hands it to every rank — torch.distributed broadcast, MPI, a file) or provided by the caller.

@@ -26,6 +26,11 @@ class nvtb_col_t(Structure):
     _fields_ = [("data", c_void_p), ("validity", c_void_p), ("dtype", c_int32), ("_pad", c_int32)]
 
 
+class nvtb_gb_chunk_t(Structure):
+    _fields_ = [("codes", c_void_p), ("valid", c_void_p), ("min", c_uint64), ("span", c_uint64),
+                ("mode", c_int32), ("lo", c_int32), ("nbits", c_int32), ("_pad", c_int32)]
+
+
 class nvtb_vocab_info_t(Structure):
     _fields_ = [("n_kept", c_int64), ("n_total", c_int64), ("null_size", c_int64),
                 ("oov_size", c_int64), ("unique_size", c_int64)]
@@ -94,6 +99,15 @@ _SIGNATURES = {
     "nvtb_groupstats_create": (c_int, [POINTER(c_void_p), c_void_p, c_int64, c_void_p, c_int, c_int64, c_void_p]),
     "nvtb_groupstats_destroy": (c_int, [c_void_p]),
     "nvtb_groupstats_gather": (c_int, [c_void_p, POINTER(nvtb_col_t), c_int64, POINTER(c_int), c_int, POINTER(c_double), POINTER(c_void_p), POINTER(c_int), POINTER(c_void_p), c_void_p]),
+    "nvtb_gb_order_codes": (c_int, [POINTER(nvtb_col_t), c_int64, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "nvtb_gb_order_rows": (c_int, [POINTER(nvtb_gb_chunk_t), POINTER(c_int), c_int, c_int64, c_int, c_void_p, c_void_p, POINTER(c_int), c_void_p]),
+    "nvtb_gb_segments_count": (c_int, [c_void_p, c_int64, c_int, POINTER(c_void_p), c_int, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
+    "nvtb_gb_segments_write": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
+    "nvtb_gb_segment_ids": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
+    "nvtb_gb_gather": (c_int, [POINTER(nvtb_col_t), c_void_p, c_uint64, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    "nvtb_gb_reduce": (c_int, [POINTER(nvtb_col_t), c_void_p, c_int64, POINTER(c_void_p), POINTER(c_void_p), c_void_p]),
+    "nvtb_gb_list_rows": (c_int, [POINTER(nvtb_col_t), c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
+    "nvtb_gb_rank_stats": (c_int, [POINTER(nvtb_col_t), c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -321,6 +321,77 @@ class Dataset:
         self.cpu = True
         return self
 
+    def shuffle_by_keys(self, keys, hive_data=None, npartitions=None) -> "Dataset":
+        """A new Dataset in which every row of one key tuple sits in exactly one of `npartitions`
+        partitions (default: as many as this one), as merlin.io.Dataset.shuffle_by_keys does for
+        the reference's Groupby (nvtabular/ops/groupby.py:30-41).
+
+        A row goes to partition hash(key tuple) % P.  Numeric keys are hashed on their order codes
+        (so -0.0 and +0.0 route alike), strings on the dictionary entry (string_hash_column), so
+        equal keys route alike from every input partition; null keys route deterministically.
+        Every input partition is read once through `partitions()`, its rows are grouped by
+        destination with the stable row-ordering kernels of the Groupby operator, and an output
+        partition is the concatenation of its pieces in input-partition order: rows of one key
+        keep their input order.  String columns get one sorted dictionary per column (codes stay
+        order-preserving).  The output partitions live in HBM.  `hive_data` is accepted for API
+        compatibility; there is no hive layout here."""
+        from . import engine
+        from .dist import world
+        from .ops.fill import materialize
+        from .ops.groupby import _order_rows
+        from .ops.hash_bucket import string_hash_column
+        if world()[0] > 1:
+            raise NotImplementedError("shuffle_by_keys across ranks of torch.distributed")
+        keys = [keys] if isinstance(keys, str) else list(keys)
+        nparts = int(npartitions or self.npartitions)
+        if nparts < 1:
+            raise ValueError("npartitions must be >= 1")
+        pieces: List[List[DeviceFrame]] = [[] for _ in range(nparts)]
+        template = None
+        for part in self.partitions():
+            for name, c in part.items():
+                if c.offsets is not None:
+                    raise NotImplementedError("shuffling list columns")
+            part = DeviceFrame({k: materialize(c) for k, c in part.items()})
+            if template is None:
+                template = part
+            n = len(part)
+            if n == 0:
+                continue
+            dev = part[keys[0]].data.device
+            hcols = []
+            for k in keys:
+                c = part[k]
+                if c.is_string:
+                    hcols.append(string_hash_column(Column(c.data, c.validity, None, c.dictionary)))
+                else:
+                    codes, valid = engine.gb_order_codes(Column(c.data, c.validity, None, None, None, c.is_bool),
+                                                         torch.empty(3, dtype=torch.int64, device=dev))
+                    hcols.append(Column(codes[:n], valid))
+            dest = engine.hash_bucket(hcols, nparts, 0, np.int32)
+            stats = torch.empty(3, dtype=torch.int64, device=dev)
+            dcodes, _ = engine.gb_order_codes(Column(dest), stats)
+            lo, hi = (int(x) for x in stats[:2].cpu().numpy().view(np.uint64))
+            order, r = _order_rows([(dcodes, None, lo, hi - lo, 0, (hi - lo).bit_length())], n, dev)
+            off, g, _ = engine.gb_segments(order, r, [dcodes], None)
+            seg_dest = engine.gb_gather(Column(dest), order, r, g, 1, off).data.cpu().tolist()
+            bounds = off.cpu().tolist()
+            for j, d in enumerate(seg_dest):
+                piece_order = order[bounds[j]: bounds[j + 1]]
+                pieces[d].append(DeviceFrame({
+                    name: engine.gb_gather(c, piece_order, r, bounds[j + 1] - bounds[j], 0)
+                    for name, c in part.items()}))
+        if template is None:
+            return Dataset([DeviceFrame()])
+        dicts = {}
+        for name, c in template.items():
+            if c.is_string:
+                all_d = [p[name].dictionary for ps in pieces for p in ps]
+                dicts[name] = np.array(sorted(set().union(*[set(d.tolist()) for d in all_d])), dtype=object) \
+                    if all_d else c.dictionary
+        out = [_concat_pieces(ps, template, dicts) for ps in pieces]
+        return Dataset(out, device=self._device)
+
     def to_parquet(self, output_path, shuffle=None, out_files_per_proc=None, seed=None, **kwargs):
         """Write the (lazily transformed) dataset as parquet part files — merlin.io.Dataset.to_parquet
         as the reference's benchmark calls it (bench/examples/dask-nvtabular-criteo-benchmark.py:225-237;
@@ -378,6 +449,31 @@ class Dataset:
             tab = tab.take(pa.array(rng.permutation(len(tab))))
             pq.write_table(tab, os.path.join(output_path, f"{prefix}{f}.parquet"))
         return output_path
+
+
+def _concat_pieces(pieces: List[DeviceFrame], template: DeviceFrame, dicts) -> DeviceFrame:
+    """one output partition of shuffle_by_keys: its pieces in order, string codes remapped to the
+    column's unified dictionary (one device gather per piece)"""
+    from .column import pack_validity, unpack_validity
+    out = {}
+    dev = next(iter(template._cols.values())).data.device if len(template.columns) else None
+    for name, t in template.items():
+        datas, valids, any_null = [], [], False
+        for p in pieces:
+            c = p[name]
+            data = c.data
+            if name in dicts and len(data):
+                lut = torch.from_numpy(np.searchsorted(dicts[name], c.dictionary).astype(np.int32)).to(data.device) \
+                    if len(c.dictionary) else torch.zeros(1, dtype=torch.int32, device=data.device)
+                data = lut[data.long().clamp_(0, max(len(c.dictionary) - 1, 0))]
+            datas.append(data)
+            valids.append(unpack_validity(c.validity, len(data), data.device))
+            any_null = any_null or c.validity is not None
+        data = torch.cat(datas) if datas else torch.empty(0, dtype=t.data.dtype, device=dev)
+        validity = pack_validity(torch.cat(valids)) if any_null else None
+        col = Column(data, validity, None, dicts.get(name, t.dictionary), None, t.is_bool)
+        out[name] = col
+    return DeviceFrame(out)
 
 
 def _permute_rows(frame: DeviceFrame, perm: torch.Tensor) -> DeviceFrame:

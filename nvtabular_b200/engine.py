@@ -592,3 +592,147 @@ class GroupStats:
                 _lib.ptr_array(vptrs) if any(vptrs) else None, _lib.stream_ptr()))
             _count()
         return [Column(o, v) for o, v in zip(outs, valid)]
+
+
+# ------------------------------------------------------------- session group-by (K8, csrc/groupby.cu)
+def _bitmask(n: int, device) -> torch.Tensor:
+    """a zeroed validity bitmask of n bits in pack_validity's padding (whole 32-byte blocks)"""
+    return torch.zeros((((n + 7) // 8 + 31) // 32) * 32, dtype=torch.uint8, device=device)
+
+
+def gb_order_codes(col: Column, stats: torch.Tensor, key_valid: Optional[torch.Tensor] = None, and_key_valid=False):
+    """-> (codes uint64-as-int64[n], validity bitmask); stats (device int64[3]) receives
+    {min, max, n_valid} of the valid codes as unsigned bit patterns (nvtb_gb_order_codes)"""
+    lib = _lib.load()
+    n = col.data.numel()
+    codes = torch.empty(max(n, 1), dtype=torch.int64, device=col.data.device)
+    valid = _bitmask(n, col.data.device)
+    with _timed("groupby_codes", _in_bytes([col]) + n * 8.125):
+        _lib.check(lib.nvtb_gb_order_codes(_descs([col]), n, _ptr(codes), _ptr(valid), _ptr(key_valid),
+                                           1 if and_key_valid else 0, _ptr(stats), _lib.stream_ptr()))
+    _count(3)
+    return codes, valid
+
+
+def gb_order_rows(chunks, round_sizes: Sequence[int], n: int, row_bits: int, device) -> torch.Tensor:
+    """rows 0..n-1 ordered by the packed fields of `chunks` (nvtb_gb_order_rows): -> the sorted
+    elements (int64 bit patterns; row = element & (2^row_bits - 1))"""
+    lib = _lib.load()
+    a = torch.empty(max(n, 1), dtype=torch.int64, device=device)
+    b = torch.empty(max(n, 1), dtype=torch.int64, device=device) if round_sizes else a
+    arr = (_lib.nvtb_gb_chunk_t * max(len(chunks), 1))()
+    for i, (codes, valid, mn, span, mode, lo, nbits) in enumerate(chunks):
+        arr[i].codes = codes.data_ptr()
+        arr[i].valid = valid.data_ptr() if valid is not None else None
+        arr[i].min, arr[i].span, arr[i].mode, arr[i].lo, arr[i].nbits = mn, span, mode, lo, nbits
+    flag = c_int(0)
+    with _timed("groupby_sort", 0.0):
+        _lib.check(lib.nvtb_gb_order_rows(arr, _lib.int_array(round_sizes), len(round_sizes), n, int(row_bits),
+                                          _ptr(a), _ptr(b), byref(flag), _lib.stream_ptr()))
+    _count(1 + 4 * len(round_sizes))
+    return (b if flag.value else a)[:n]
+
+
+def gb_segments(order: torch.Tensor, row_bits: int, key_codes: Sequence[torch.Tensor],
+                key_valid: Optional[torch.Tensor]):
+    """-> (offsets int64[G + 1], G, rows with valid keys); one host read (nvtb_gb_segments_*)"""
+    lib = _lib.load()
+    n = order.numel()
+    dev = order.device
+    flags = torch.empty(max((n + 7) // 8, 1), dtype=torch.uint8, device=dev)
+    tiles = torch.empty(max((n + 2047) // 2048, 1), dtype=torch.int32, device=dev)
+    counts = (c_int64 * 2)()
+    with _timed("groupby_segments", n * (8.0 + 8 * len(key_codes))):
+        _lib.check(lib.nvtb_gb_segments_count(_ptr(order), n, int(row_bits),
+                                              _lib.ptr_array([k.data_ptr() for k in key_codes]), len(key_codes),
+                                              _ptr(key_valid), _ptr(flags), _ptr(tiles), counts, _lib.stream_ptr()))
+        g, kept = int(counts[0]), int(counts[1])
+        off = torch.empty(g + 1, dtype=torch.int64, device=dev)
+        _lib.check(lib.nvtb_gb_segments_write(_ptr(flags), _ptr(tiles), n, g, kept, _ptr(off), _lib.stream_ptr()))
+    _count(3)
+    return off, g, kept
+
+
+def gb_segment_ids(off: torch.Tensor, n_groups: int, n: int) -> torch.Tensor:
+    lib = _lib.load()
+    gid = torch.empty(max(n, 1), dtype=torch.int64, device=off.device)
+    _lib.check(lib.nvtb_gb_segment_ids(_ptr(off), n_groups, n, _ptr(gid), _lib.stream_ptr()))
+    _count()
+    return gid
+
+
+def gb_gather(col: Column, order: Optional[torch.Tensor], row_bits: int, m: int, which: int = 0,
+              off: Optional[torch.Tensor] = None) -> Column:
+    """data + validity of `col` at row(i) (which 0), at the first (1) or last (2) position of every
+    segment; row(p) = order[p] & (2^row_bits - 1), or p without an order (nvtb_gb_gather)"""
+    lib = _lib.load()
+    dev = col.data.device
+    out = torch.empty(m, dtype=col.data.dtype, device=dev)
+    valid = _bitmask(m, dev) if col.validity is not None else None
+    with _timed("groupby_gather", m * (col.data.element_size() * 2 + (8 if order is not None else 0))):
+        _lib.check(lib.nvtb_gb_gather(_descs([col]), _ptr(order), (1 << row_bits) - 1, _ptr(off), m, which,
+                                      _ptr(out), _ptr(valid), _lib.stream_ptr()))
+    _count()
+    return Column(out, valid, None, col.dictionary, None, col.is_bool)
+
+
+def gb_reduce(col: Column, off: torch.Tensor, n_groups: int, aggs: Sequence[str]):
+    """{agg: Column} for the aggs of {count, sum, mean, var, std, min, max} over every segment of a
+    column in group order (nvtb_gb_reduce: fp64, fixed order)"""
+    lib = _lib.load()
+    dev = col.data.device
+    names = ("count", "sum", "mean", "var", "std", "min", "max")
+    outs, ptrs = {}, []
+    for a in names:
+        if a in aggs:
+            dt = torch.int32 if a == "count" else (col.data.dtype if a in ("min", "max") else torch.float32)
+            outs[a] = torch.empty(max(n_groups, 1), dtype=dt, device=dev)
+            ptrs.append(outs[a].data_ptr())
+        else:
+            ptrs.append(None)
+    is_int = not col.data.dtype.is_floating_point
+    valid = {a: _bitmask(n_groups, dev) for a in ("min", "max") if a in aggs and is_int}
+    vptrs = _lib.ptr_array([valid[a].data_ptr() if a in valid else None for a in ("min", "max")]) if valid else None
+    with _timed("groupby_reduce", _in_bytes([col]) + n_groups * (8 + 4 * len(outs))):
+        _lib.check(lib.nvtb_gb_reduce(_descs([col]), _ptr(off), n_groups, _lib.ptr_array(ptrs), vptrs,
+                                      _lib.stream_ptr()))
+    _count(2)
+    res = {}
+    for a, t in outs.items():
+        if a in ("min", "max"):
+            res[a] = Column(t[:n_groups], valid.get(a), None, col.dictionary, None, col.is_bool)
+        else:
+            res[a] = Column(t[:n_groups])
+    return res
+
+
+def gb_rank_stats(col: Column, codes: torch.Tensor, codes_valid: torch.Tensor, order: torch.Tensor, row_bits: int,
+                  off: torch.Tensor, n_groups: int, median: bool, nunique: bool):
+    """-> (median float32[G] | None, nunique int32[G] | None) (nvtb_gb_rank_stats)"""
+    lib = _lib.load()
+    dev = col.data.device
+    med = torch.empty(max(n_groups, 1), dtype=torch.float32, device=dev) if median else None
+    nun = torch.empty(max(n_groups, 1), dtype=torch.int32, device=dev) if nunique else None
+    with _timed("groupby_rank", order.numel() * 16.0):
+        _lib.check(lib.nvtb_gb_rank_stats(_descs([col]), _ptr(codes), _ptr(codes_valid), _ptr(order),
+                                          (1 << row_bits) - 1, _ptr(off), n_groups, _ptr(med), _ptr(nun),
+                                          _lib.stream_ptr()))
+    _count()
+    return (med[:n_groups] if med is not None else None), (nun[:n_groups] if nun is not None else None)
+
+
+def gb_list_rows(leaves: Column, lo: torch.Tensor, hi: torch.Tensor) -> Column:
+    """a list column whose row g holds leaves[lo[g]:hi[g]] (nvtb_gb_list_rows)"""
+    lib = _lib.load()
+    m = lo.numel()
+    dev = leaves.data.device
+    off = torch.empty(m + 1, dtype=torch.int64, device=dev)
+    total = c_int64(0)
+    _lib.check(lib.nvtb_gb_list_rows(_descs([leaves]), _ptr(lo), _ptr(hi), m, _ptr(off), None, None, byref(total),
+                                     _lib.stream_ptr()))
+    out = torch.empty(total.value, dtype=leaves.data.dtype, device=dev)
+    valid = _bitmask(total.value, dev) if leaves.validity is not None else None
+    _lib.check(lib.nvtb_gb_list_rows(_descs([leaves]), _ptr(lo), _ptr(hi), m, _ptr(off), _ptr(out), _ptr(valid),
+                                     byref(total), _lib.stream_ptr()))
+    _count(2)
+    return Column(out, valid, off, leaves.dictionary, None, leaves.is_bool)

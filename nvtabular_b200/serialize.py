@@ -240,6 +240,13 @@ def _registry():
             lambda p, s, adir: ops.HashBucket(num_buckets=p["num_buckets"])),
         "nvtabular.ops.join_groupby.JoinGroupby": (ops.JoinGroupby, _join_groupby_to, _join_groupby_from),
         "nvtabular.ops.target_encoding.TargetEncoding": (ops.TargetEncoding, _target_encoding_to, _target_encoding_from),
+        "nvtabular.ops.groupby.Groupby": (
+            ops.Groupby, lambda op, adir: ({"groupby_cols": list(op.groupby_cols), "sort_cols": list(op.sort_cols),
+                                            "aggs": {k: list(v) for k, v in op.aggs.items()},
+                                            "name_sep": op.name_sep, "ascending": op.ascending}, {}),
+            lambda p, s, adir: ops.Groupby(groupby_cols=p.get("groupby_cols"), sort_cols=p.get("sort_cols"),
+                                           aggs=p.get("aggs", "list"), name_sep=p.get("name_sep", "_"),
+                                           ascending=p.get("ascending", True))),
     }
 
 

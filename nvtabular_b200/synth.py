@@ -128,3 +128,25 @@ def hashbucket_frame(rows: int, ncols: int = 40, n_ids: int = 100_000_000, seed:
         k.mul_(m2)
         cols[f"K{j + 1}"] = Column(k)
     return DeviceFrame(cols)
+
+
+def session_frame(rows: int, seed: int = 1234, device="cuda", mean_length: float = 10.0):
+    """A synthetic session table of `rows` rows, grouped by nothing: session_id (int64, lengths
+    drawn from a Zipf-like power law with about rows / mean_length sessions, rows shuffled),
+    item_id (int32), ts (int64 seconds near 1.7e9), price (float32).  -> (DeviceFrame, sessions)."""
+    g = torch.Generator(device=device)
+    g.manual_seed(seed)
+    n_sess = max(1, int(rows / mean_length))
+    # power-law lengths: a Pareto tail, scaled to the row count
+    u = torch.rand(n_sess, generator=g, device=device, dtype=torch.float64)
+    w = u.clamp_min(1e-12).pow(-1.0 / 1.2)
+    lens = torch.floor(w / w.sum() * (rows - n_sess)).to(torch.int64) + 1
+    lens[0] += rows - int(lens.sum().item())
+    sid = torch.repeat_interleave(torch.arange(n_sess, dtype=torch.int64, device=device), lens)
+    perm = torch.randperm(rows, generator=g, device=device)
+    sid = sid[perm].contiguous()
+    item = torch.randint(0, 1 << 20, (rows,), generator=g, device=device, dtype=torch.int32)
+    ts = 1_700_000_000 + torch.randint(0, 1 << 24, (rows,), generator=g, device=device, dtype=torch.int64)
+    price = torch.rand(rows, generator=g, device=device, dtype=torch.float32) * 100
+    return DeviceFrame({"session_id": Column(sid), "item_id": Column(item), "ts": Column(ts),
+                        "price": Column(price)}), n_sess
