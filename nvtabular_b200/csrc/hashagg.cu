@@ -1638,10 +1638,10 @@ int nvtb_hashagg_reset(nvtb_hashagg_t* h, void* stream) {
   }
   special_init_kernel<<<1, 32, 0, st>>>(h->ctr, h->special_vals, h->n_agg);
   NVTB_LAUNCH_OK();
+  h->stage_hint = std::max<int64_t>(h->stage_hint, h->rows_total);   // the fit that just ended
   h->u_known = 0;
   h->rows_total = 0;
-  h->stage_hint = std::max<int64_t>(h->stage_hint, h->rows_total);
-  h->stage_rows = 0;           // batches still waiting belong to the fit that is being discarded
+  h->stage_rows = 0;          // batches still waiting belong to the fit that is being discarded
   h->mailbox_valid = false;
   return NVTB_OK;
 }

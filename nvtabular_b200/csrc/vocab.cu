@@ -476,11 +476,15 @@ lookup_build_packed_kernel(const uint64_t* __restrict__ p, int64_t n, unsigned l
 // slice-wise build of a large narrow lookup.  One random insert per key into a multi-GB table is
 // one DRAM-resident atomic per key (every warp waiting on its CAS, far from the DRAM peak).  Instead the (position, key) items are partitioned by the table slice
 // their home bucket lies in (order-free: shared-memory counts, one reservation per tile and
-// slice), and one CTA then zero-fills and fills ITS slice: the slice stays in the L2 while it
-// is built, the atomics are L2 hits, and every table line reaches HBM exactly once.
+// slice), and one CTA then builds ITS slice: in shared memory when the slice is 8192 buckets
+// (slice_build_smem_kernel), else in place in the L2 (slice_build_kernel).  Every table line
+// reaches HBM once.
 // ---------------------------------------------------------------------------------------
 constexpr int kSlThreads = 512;
-constexpr int kSlTile = 4096;                      // items per tile of the scatter (32 KB staged): 2 CTAs per SM
+// items per tile of the scatter (128 KB staged, one CTA per SM): with up to 8192 slices a tile
+// puts several items into each slice's run, so a run grows by whole sectors more often and there
+// are fewer cursor reservations per item
+constexpr int kSlTile = 16384;
 
 __device__ __forceinline__ uint32_t slice_of(uint32_t key, uint32_t bmask, int lg_slice) {
   return (table_mix32(key) & bmask) >> lg_slice;
@@ -516,7 +520,7 @@ slice_scan_kernel(const uint32_t* __restrict__ total, int P, uint32_t* __restric
 }
 
 // items[...] = ((pos + 1) << 32) | key, grouped by slice
-static __global__ void __launch_bounds__(kSlThreads, 2)
+static __global__ void __launch_bounds__(kSlThreads, 1)
 slice_scatter_kernel(const uint64_t* __restrict__ p, int64_t n, uint32_t bmask, int lg_slice, int P,
                      uint32_t* __restrict__ cursor, uint64_t* __restrict__ items) {
   extern __shared__ __align__(16) unsigned char sl_raw[];
@@ -524,7 +528,7 @@ slice_scatter_kernel(const uint64_t* __restrict__ p, int64_t n, uint32_t bmask, 
   uint32_t* cnt = reinterpret_cast<uint32_t*>(stage + kSlTile);                 // [P]
   uint32_t* delta = cnt + P;                                                    // [P]
   __shared__ uint32_t ws[kSlThreads / 32 + 1];
-  constexpr int kPer = kSlTile / kSlThreads;                                    // 16 items per thread
+  constexpr int kPer = kSlTile / kSlThreads;                                    // 32 items per thread
   const int64_t n_tiles = (n + kSlTile - 1) / kSlTile;
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     for (int d = threadIdx.x; d < P; d += kSlThreads) cnt[d] = 0u;
@@ -581,6 +585,63 @@ slice_build_kernel(const uint64_t* __restrict__ items, const uint32_t* __restric
   for (uint32_t i = s + threadIdx.x; i < e; i += blockDim.x) {
     const unsigned long long want = items[i];
     narrow_claim(slots, (int64_t)(table_mix32((uint32_t)want) & bmask), (int64_t)bmask + 1, want);
+  }
+}
+
+// One CTA per slice of kSliceBuckets buckets, built in shared memory: a claim counter per bucket
+// (32 KB) and, per slot, the index (+ 1) of the item that claimed it within the slice's run (16
+// bits: a slice holds at most 4 * kSliceBuckets items; 64 KB).  An item takes the next slot of its
+// home bucket, or of the first bucket after it in the slice that is not yet full — the placement
+// narrow_claim makes in the table.  Then each table slot is written once, in order: the item it
+// holds (re-read from the run, which this CTA has just read) or 0.  The inserts are shared-memory
+// atomicAdds, and the table is written without a zero-fill pass or a read-modify-write of its lines.
+constexpr int kSlBuildThreads = 1024;
+constexpr int kSlBuildSlots = 4 * (int)kSliceBuckets;
+constexpr int kSlBuildSmem = (int)kSliceBuckets * 4 + kSlBuildSlots * 2;    // 96 KB: 2 CTAs per SM
+
+static __global__ void __launch_bounds__(kSlBuildThreads, 2)
+slice_build_smem_kernel(const uint64_t* __restrict__ items, const uint32_t* __restrict__ starts,
+                        unsigned long long* __restrict__ slots, uint32_t bmask) {
+  extern __shared__ __align__(16) uint32_t sb_fill[];                         // [kSliceBuckets]
+  unsigned short* sb_item = reinterpret_cast<unsigned short*>(sb_fill + kSliceBuckets);   // [kSlBuildSlots]
+  constexpr uint32_t kBm = (uint32_t)kSliceBuckets - 1;
+  constexpr int kUnroll = 4;
+  const int sl = blockIdx.x;
+  for (int i = threadIdx.x; i < (int)kSliceBuckets / 4; i += kSlBuildThreads)
+    reinterpret_cast<uint4*>(sb_fill)[i] = make_uint4(0u, 0u, 0u, 0u);
+  __syncthreads();
+  const uint32_t s = starts[sl], e = starts[sl + 1];
+  for (uint32_t i0 = s + threadIdx.x; i0 < e; i0 += kUnroll * kSlBuildThreads) {
+    uint32_t key[kUnroll];
+#pragma unroll
+    for (int k = 0; k < kUnroll; ++k) {
+      const uint32_t i = i0 + k * kSlBuildThreads;
+      key[k] = i < e ? (uint32_t)items[i] : 0u;
+    }
+#pragma unroll
+    for (int k = 0; k < kUnroll; ++k) {
+      const uint32_t i = i0 + k * kSlBuildThreads;
+      if (i >= e) continue;
+      uint32_t b = (table_mix32(key[k]) & bmask) & kBm;
+      uint32_t j;
+      while ((j = atomicAdd(sb_fill + b, 1u)) >= 4u) b = (b + 1) & kBm;
+      sb_item[4 * b + j] = (unsigned short)(i - s + 1);
+    }
+  }
+  __syncthreads();
+  unsigned long long* base = slots + (int64_t)sl * kSlBuildSlots;
+  for (int q0 = threadIdx.x; q0 < kSlBuildSlots; q0 += kUnroll * kSlBuildThreads) {
+    uint32_t r[kUnroll];
+    unsigned long long w[kUnroll];
+#pragma unroll
+    for (int k = 0; k < kUnroll; ++k) {
+      const int q = q0 + k * kSlBuildThreads;
+      r[k] = (uint32_t)(q & 3) < sb_fill[q >> 2] ? (uint32_t)sb_item[q] : 0u;
+    }
+#pragma unroll
+    for (int k = 0; k < kUnroll; ++k) w[k] = r[k] ? items[s + r[k] - 1] : 0ull;
+#pragma unroll
+    for (int k = 0; k < kUnroll; ++k) base[q0 + k * kSlBuildThreads] = w[k];
   }
 }
 
@@ -1029,6 +1090,7 @@ static int finish_packed_vocab(nvtb_vocab* v, uint64_t* sorted, int64_t n, const
     const int g1 = plain_grid(n_keep);
     if (sliced) {
       static bool sl_attrs = false;
+      const bool smem_build = slice_buckets == kSliceBuckets;
       const int P = (int)n_slices;                                   // a power of two <= 8192
       int lg_slice = 0;
       while (((int64_t)1 << lg_slice) < slice_buckets) ++lg_slice;
@@ -1036,6 +1098,7 @@ static int finish_packed_vocab(nvtb_vocab* v, uint64_t* sorted, int64_t n, const
       if (!sl_attrs) {
         NVTB_CUDA_OK(cudaFuncSetAttribute(slice_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 4 * kSliceParts));
         NVTB_CUDA_OK(cudaFuncSetAttribute(slice_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, scatter_smem));
+        NVTB_CUDA_OK(cudaFuncSetAttribute(slice_build_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSlBuildSmem));
         sl_attrs = true;
       }
       uint32_t* meta = nullptr;                                      // total[P] | starts[P + 1] | cursor[P]
@@ -1050,10 +1113,14 @@ static int finish_packed_vocab(nvtb_vocab* v, uint64_t* sorted, int64_t n, const
       slice_scan_kernel<<<1, kSlThreads, 2 * 4 * P, st>>>(meta, P, meta + P, meta + 2 * P + 1);
       NVTB_LAUNCH_OK();
       const int64_t tiles = (n_keep + kSlTile - 1) / kSlTile;
-      slice_scatter_kernel<<<(int)std::min<int64_t>(tiles, 2 * sms), kSlThreads, kSlTile * 8 + 2 * 4 * P, st>>>(
+      slice_scatter_kernel<<<(int)std::min<int64_t>(tiles, sms), kSlThreads, kSlTile * 8 + 2 * 4 * P, st>>>(
           sorted, n_keep, bmask, lg_slice, P, meta + 2 * P + 1, items);
       NVTB_LAUNCH_OK();
-      slice_build_kernel<<<P, 1024, 0, st>>>(items, meta + P, reinterpret_cast<unsigned long long*>(v->t.slots), bmask, lg_slice);
+      if (smem_build)
+        slice_build_smem_kernel<<<P, kSlBuildThreads, kSlBuildSmem, st>>>(items, meta + P,
+                                                                          reinterpret_cast<unsigned long long*>(v->t.slots), bmask);
+      else
+        slice_build_kernel<<<P, 1024, 0, st>>>(items, meta + P, reinterpret_cast<unsigned long long*>(v->t.slots), bmask, lg_slice);
       NVTB_LAUNCH_OK();
       NVTB_CUDA_OK(cudaFreeAsync(items, st));
       NVTB_CUDA_OK(cudaFreeAsync(meta, st));
