@@ -49,7 +49,8 @@ typedef enum {
   NVTB_ENOMEM = -2,  /* device allocation failed                          */
   NVTB_ECUDA = -3,   /* a CUDA runtime call or kernel launch failed       */
   NVTB_ESTATE = -4,  /* handle used in the wrong phase                    */
-  NVTB_ENCCL = -5    /* an NCCL call failed / NCCL is not loadable         */
+  NVTB_ENCCL = -5,   /* an NCCL call failed / NCCL is not loadable         */
+  NVTB_EIO = -6      /* a file could not be written (the path is in the message) */
 } nvtb_status_t;
 
 typedef enum {
@@ -331,6 +332,59 @@ int nvtb_vocab_info(const nvtb_vocab_t* v, nvtb_vocab_info_t* info_host);
 /* copy the kept keys / sizes in label order into caller device arrays */
 int nvtb_vocab_export(const nvtb_vocab_t* v, int64_t* keys_out,
                       int64_t* sizes_out, void* stream);
+
+/* ---- Categorify artefact files (csrc/artifacts.cu, host only) ---------------------------
+ * meta.<col>.parquet and unique.<col>.parquet (reference nvtabular/ops/categorify.py:731-822)
+ * written by library threads instead of pandas / pyarrow calls under the GIL.  The files are
+ * what DataFrame.to_parquet(compression=None) writes, reduced to what pandas needs to read them
+ * back: one row group, PLAIN, uncompressed v1 data pages of about 1 MiB per OPTIONAL column (no
+ * dictionary pages, no statistics), and the `pandas` schema metadata, which carries the RangeIndex of the
+ * labels.  Column types: INT32, INT64, FLOAT, DOUBLE, and BYTE_ARRAY + UTF8 for the meta
+ * file's `kind` column.
+ *
+ * nvtb_parquet_write: host arrays -> one file.  cols_host[c].data holds n values of dtype
+ * I32 | I64 | F32 | F64.  pandas_meta: the JSON stored under the `pandas` key (may be NULL).
+ * page_rows: values per data page, 0 = pages of about 1 MiB. */
+typedef struct {
+  const char* name;
+  const void* data;   /* host */
+  int32_t dtype;      /* nvtb_dtype_t */
+  int32_t _pad;
+} nvtb_pq_col_t;
+int nvtb_parquet_write(const char* path, const nvtb_pq_col_t* cols_host, int ncols, int64_t n,
+                       const char* pandas_meta, int64_t page_rows);
+/* meta.<col>.parquet of a vocabulary from its (host) info: kind = pad, null, oov, unique;
+ * offset = 0, 1, 2, 2 + oov_count; num_indices = 1, 1, oov_count, n_kept; with_observed != 0
+ * adds num_observed = 0, null_size, oov_size, unique_size.  oov_count = num_buckets or 1. */
+int nvtb_parquet_write_meta(const char* path, int64_t oov_count, const nvtb_vocab_info_t* info_host,
+                            int with_observed, const char* pandas_meta);
+/* An asynchronous batch of vocabulary files.  begin starts `threads` writer threads (>= 1).
+ * submit_vocab returns at once and never waits for the device.  Jobs run as their vocabularies'
+ * builds finish (the event the enqueued build records, or, for a handle without one, an event
+ * recorded here on `stream`), not in submission order: a writer thread takes the first queued
+ * job whose event has fired, reads the vocabulary's scalars, copies the kept keys / sizes to the host
+ * through library-owned pinned memory on a stream of its own, decodes the keys and writes
+ *   meta_path    kind (pad, null, oov, unique), offset, num_indices [, num_observed when
+ *                size_name != NULL]; meta_pandas is its `pandas` metadata;
+ *   unique_path  (may be NULL) key_name [, size_name] with the kept rows, when the handle saw at
+ *                least one key and unique_max_rows < 0 or n_kept <= unique_max_rows; its
+ *                `pandas` metadata is unique_pandas_head + decimal(index_start + n_kept) +
+ *                unique_pandas_tail (the stop of the RangeIndex is only known then).
+ * key_dtype is the dtype of the written keys: I32 | I64 (int keys, written as they are) or
+ * F32 | F64 (float keys: the order-preserving int64 image of a float64, k >= 0 ? k :
+ * k ^ INT64_MAX, turned back into the float64 and cast).  oov_count = num_buckets or 1.
+ * join waits for every job, stops the threads, frees the handle, and returns the status of the
+ * first submitted job that failed (nvtb_last_error() names its path).  The vocabulary handles
+ * must outlive the join. */
+typedef struct nvtb_artifacts nvtb_artifacts_t;
+int nvtb_artifacts_begin(nvtb_artifacts_t** out, int threads);
+int nvtb_artifacts_submit_vocab(nvtb_artifacts_t* h, const nvtb_vocab_t* v, const char* meta_path,
+                                const char* meta_pandas, const char* unique_path,
+                                int64_t unique_max_rows, const char* key_name, int key_dtype,
+                                const char* size_name, int64_t index_start, int64_t oov_count,
+                                const char* unique_pandas_head, const char* unique_pandas_tail,
+                                void* stream);
+int nvtb_artifacts_join(nvtb_artifacts_t* h);
 
 /* _encode (reference nvtabular/ops/categorify.py:1558-1807), without the
  * join + sort: label = null_label for null rows; first_label + position for

@@ -31,6 +31,10 @@ class nvtb_gb_chunk_t(Structure):
                 ("mode", c_int32), ("lo", c_int32), ("nbits", c_int32), ("_pad", c_int32)]
 
 
+class nvtb_pq_col_t(Structure):
+    _fields_ = [("name", c_char_p), ("data", c_void_p), ("dtype", c_int32), ("_pad", c_int32)]
+
+
 class nvtb_vocab_info_t(Structure):
     _fields_ = [("n_kept", c_int64), ("n_total", c_int64), ("null_size", c_int64),
                 ("oov_size", c_int64), ("unique_size", c_int64)]
@@ -79,6 +83,12 @@ _SIGNATURES = {
     "nvtb_vocab_destroy": (c_int, [c_void_p]),
     "nvtb_vocab_info": (c_int, [c_void_p, POINTER(nvtb_vocab_info_t)]),
     "nvtb_vocab_export": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nvtb_parquet_write": (c_int, [c_char_p, POINTER(nvtb_pq_col_t), c_int, c_int64, c_char_p, c_int64]),
+    "nvtb_parquet_write_meta": (c_int, [c_char_p, c_int64, POINTER(nvtb_vocab_info_t), c_int, c_char_p]),
+    "nvtb_artifacts_begin": (c_int, [POINTER(c_void_p), c_int]),
+    "nvtb_artifacts_submit_vocab": (c_int, [c_void_p, c_void_p, c_char_p, c_char_p, c_char_p, c_int64, c_char_p, c_int,
+                                            c_char_p, c_int64, c_int64, c_char_p, c_char_p, c_void_p]),
+    "nvtb_artifacts_join": (c_int, [c_void_p]),
     "nvtb_encode_apply": (c_int, [c_void_p, POINTER(nvtb_col_t), c_int64, c_int64, c_int64, c_int64, c_uint64, POINTER(nvtb_col_t), c_int, c_void_p, c_int, c_void_p]),
     "nvtb_comm_available": (c_int, []),
     "nvtb_comm_unique_id": (c_int, [c_void_p]),

@@ -953,7 +953,7 @@ static void pin_release(VocabScalars* p) {
   g_pin_free.push_back((int)(p - g_pin_slab));
 }
 
-// serialised: a host thread writing the artefact files and the thread running transform may
+// serialised: the artefact writer threads (artifacts.cu) and the thread running transform may
 // both ask for the scalars of the same vocabulary first
 static std::mutex g_fin_mu;
 
@@ -967,9 +967,17 @@ static void vocab_apply(nvtb_vocab* v, const VocabScalars& h) {
 }
 
 static int vocab_finalize(nvtb_vocab* v) {
+  cudaEvent_t ev = nullptr;
+  {
+    std::lock_guard<std::mutex> lk(g_fin_mu);
+    if (!v->pending) return NVTB_OK;
+    ev = v->ev;
+  }
+  // wait without the lock: a writer thread waiting for a large build must not hold up the
+  // finalize of a vocabulary that is already built (the event lives as long as the handle)
+  NVTB_CUDA_OK(cudaEventSynchronize(ev));
   std::lock_guard<std::mutex> lk(g_fin_mu);
   if (!v->pending) return NVTB_OK;
-  NVTB_CUDA_OK(cudaEventSynchronize(v->ev));
   vocab_apply(v, *v->h_sc);
   v->pending = false;
   if (v->d_sc) { cudaFreeAsync(v->d_sc, 0); v->d_sc = nullptr; }
@@ -977,6 +985,10 @@ static int vocab_finalize(nvtb_vocab* v) {
   v->h_sc = nullptr;
   return NVTB_OK;
 }
+
+// the event that completes v's enqueued build (its kept rows are final once it has fired), or
+// nullptr when the build was finished on the host or the handle was made by from_arrays
+cudaEvent_t vocab_build_event(const nvtb_vocab* v) { return v->ev; }
 
 // enqueue the readback of the device scalars; falls back to a blocking read when the
 // pinned pool is exhausted

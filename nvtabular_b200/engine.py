@@ -6,6 +6,7 @@ No arithmetic happens in Python on row data; torch is used to allocate output
 buffers and to read back O(#columns) scalars.
 """
 import ctypes
+import os
 from ctypes import byref, c_int, c_int64, c_void_p
 from typing import List, Optional, Sequence
 
@@ -492,6 +493,74 @@ class Vocab:
                 _ptr(out), code, _lib.stream_ptr()))
         _count()
         return out
+
+
+# ------------------------------------------------------------ artefact files
+def _path(p) -> bytes:
+    return os.fsencode(str(p))
+
+
+def parquet_write(path, columns, pandas_meta: Optional[bytes] = None, page_rows: int = 0):
+    """[(name, 1-d numpy array of int32 | int64 | float32 | float64)] of one length -> a parquet
+    file (nvtb_parquet_write: PLAIN, uncompressed pages of `page_rows` values, 0 = about 1 MiB;
+    host only, no device)"""
+    lib = _lib.load()
+    arrays = [(name, np.ascontiguousarray(a)) for name, a in columns]
+    n = len(arrays[0][1]) if arrays else 0
+    cols = (_lib.nvtb_pq_col_t * max(len(arrays), 1))()
+    for i, (name, a) in enumerate(arrays):
+        if a.dtype not in _NP2CODE or a.dtype in (np.dtype("uint8"), np.dtype("bool")) or a.ndim != 1 or len(a) != n:
+            raise TypeError(f"parquet_write: column {name!r} must be a 1-d int32/int64/float32/float64 "
+                            f"array of {n} values, got {a.dtype} {a.shape}")
+        cols[i].name = str(name).encode()
+        cols[i].data = a.ctypes.data if n else None
+        cols[i].dtype = _NP2CODE[a.dtype]
+    _lib.check(lib.nvtb_parquet_write(_path(path), cols, len(arrays), n, pandas_meta, int(page_rows)))
+
+
+def parquet_write_meta(path, oov_count: int, n_kept: int, null_size=0, oov_size=0, unique_size=0,
+                       with_observed=True, pandas_meta: bytes = b""):
+    """meta.<col>.parquet of a vocabulary (nvtb_parquet_write_meta; host only)"""
+    lib = _lib.load()
+    info = _lib.nvtb_vocab_info_t(int(n_kept), 0, int(null_size), int(oov_size), int(unique_size))
+    _lib.check(lib.nvtb_parquet_write_meta(_path(path), int(oov_count), byref(info), 1 if with_observed else 0,
+                                           pandas_meta))
+
+
+class ArtifactWriter:
+    """A batch of vocabulary files written by library threads (nvtb_artifacts_*).  submit_vocab
+    returns without waiting for the device; join() waits for every file, stops the threads and
+    raises NvtbError (naming the path) if a write failed."""
+
+    def __init__(self, threads: int = 4):
+        self.lib = _lib.load()
+        self.h = c_void_p()
+        _lib.check(self.lib.nvtb_artifacts_begin(byref(self.h), int(threads)))
+        self._vocabs = []            # the handles must outlive the join
+
+    def submit_vocab(self, vocab: "Vocab", meta_path, meta_pandas: bytes, unique_path, unique_max_rows: int,
+                     key_name: str, key_dtype, size_name: Optional[str], index_start: int, oov_count: int,
+                     unique_pandas_head: bytes, unique_pandas_tail: bytes):
+        self._vocabs.append(vocab)
+        _lib.check(self.lib.nvtb_artifacts_submit_vocab(
+            self.h, vocab.h, _path(meta_path), meta_pandas, _path(unique_path) if unique_path else None,
+            int(unique_max_rows), key_name.encode(), dtype_code(key_dtype),
+            size_name.encode() if size_name is not None else None, int(index_start), int(oov_count),
+            unique_pandas_head, unique_pandas_tail, _lib.stream_ptr()))
+
+    def join(self):
+        h, self.h = self.h, c_void_p()
+        if h.value:
+            rc = self.lib.nvtb_artifacts_join(h)
+            self._vocabs = []
+            _lib.check(rc)
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None) is not None and self.h.value:
+                self.lib.nvtb_artifacts_join(self.h)
+        except Exception:
+            pass
 
 
 def pairs_lower_bounds(pairs: torch.Tensor, bounds: torch.Tensor) -> torch.Tensor:

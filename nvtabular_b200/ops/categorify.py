@@ -30,6 +30,7 @@ from .keyspace import ComboKeySpace, KeySpace, _leaf
 
 PAD_OFFSET, NULL_OFFSET, OOV_OFFSET = 0, 1, 2   # categorify.py:51-55
 EAGER_ARTIFACT_ROWS = 1 << 20                   # larger vocabularies are written lazily
+WRITER_THREADS = 4                              # library threads writing the artefact files of a fit
 
 
 def _artifacts_mode() -> str:
@@ -37,9 +38,10 @@ def _artifacts_mode() -> str:
 
     eager  every meta.<col>.parquet and the unique.<col>.parquet of every vocabulary up to
            2^20 keys is written DURING fit, like the reference (whose only fitted state IS those
-           files).  The small vocabularies are built first and their keys / sizes copied to
-           pinned host memory while the GPU goes on with the builds of the large columns;
-           the files are then written (pyarrow, no dictionary pages) under that GPU work.
+           files).  The small vocabularies are built first; library threads
+           (engine.ArtifactWriter) copy their keys / sizes to the host and write the files while
+           the GPU goes on with the builds of the large columns, and fit_finalize joins those
+           threads before it returns.
            Larger vocabulary files are written when their path is first read
            (`op.categories[name]`, `Workflow.save`, `set_storage_path`).
     lazy   nothing until a path is read."""
@@ -73,16 +75,22 @@ def _pandas_meta(columns, index_start, n):
         "pandas_version": pd.__version__}).encode()
 
 
+def _pandas_meta_parts(columns, index_start):
+    """_pandas_meta cut around the stop of the RangeIndex -> (head, tail), for a writer that only
+    learns the row count later: the metadata is head + str(index_start + n) + tail"""
+    text = _pandas_meta(columns, index_start, 0)
+    stop = b'"stop": %d' % int(index_start)
+    head, tail = text.split(stop)           # column names are escaped: they cannot hold this
+    return head + b'"stop": ', tail
+
+
 def _write_numeric_parquet(path, arrays, index_start):
     """{name: numpy array} -> parquet that pandas reads back as a frame with
     RangeIndex(index_start, ...): what df.to_parquet(compression=None) writes, minus the pandas
-    conversion and the dictionary pages (each slower than the write itself)."""
-    import pyarrow as pa
-    import pyarrow.parquet as pq
+    conversion and the dictionary pages.  Written by the library (engine.parquet_write)."""
     n = len(next(iter(arrays.values()))) if arrays else 0
-    tb = pa.table({k: pa.array(v) for k, v in arrays.items()})
-    tb = tb.replace_schema_metadata({b"pandas": _pandas_meta([(k, v.dtype) for k, v in arrays.items()], index_start, n)})
-    pq.write_table(tb, path, compression=None, use_dictionary=False)
+    engine.parquet_write(path, list(arrays.items()),
+                         _pandas_meta([(k, v.dtype) for k, v in arrays.items()], index_start, n))
 
 
 def _make_name(*args, sep="_"):
@@ -112,7 +120,7 @@ class FittedVocab:
         self.index_start = OOV_OFFSET + oov_count if index_start is None else index_start
         self.path = None
         self._written = False
-        self._host = None          # (keys, sizes | None, event): pinned copies queued by prefetch_host
+        self._queued = None        # (base_path, force) of files queued on an ArtifactWriter
 
     @property
     def n_kept(self):
@@ -123,32 +131,7 @@ class FittedVocab:
         """rows of unique.<name>.parquet (an empty input writes one null row)"""
         return 1 if self.vocab.n_total == 0 else self.vocab.n_kept
 
-    def prefetch_host(self):
-        """Queue the device -> pinned-host copy of the kept keys / sizes (no host wait beyond this
-        vocabulary's own build).  Called for the small vocabularies before the large builds are
-        queued, so that their files can be written while the GPU is still busy."""
-        if self._host is not None or _artifacts_lazy() or not torch.cuda.is_available():
-            return
-        n = self.vocab.n_kept
-        if n == 0 or n > EAGER_ARTIFACT_ROWS:
-            return
-        keys, sizes = self.vocab.export(with_sizes=self.has_sizes)
-        hk = torch.empty(n, dtype=torch.int64, pin_memory=True)
-        hk.copy_(keys, non_blocking=True)
-        hs = None
-        if sizes is not None:
-            hs = torch.empty(n, dtype=torch.int64, pin_memory=True)
-            hs.copy_(sizes, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._host = (hk, hs, ev, keys, sizes)     # the device arrays stay alive until the copy is done
-
     def _host_arrays(self):
-        if self._host is not None:
-            hk, hs, ev, _, _ = self._host
-            ev.synchronize()
-            self._host = None
-            return hk.numpy(), (hs.numpy() if hs is not None else None)
         keys, sizes = self.vocab.export(with_sizes=self.has_sizes)
         return keys.cpu().numpy(), (sizes.cpu().numpy() if sizes is not None else None)
 
@@ -165,55 +148,91 @@ class FittedVocab:
         df.index = pd.RangeIndex(self.index_start, self.index_start + len(df))
         return df
 
-    def meta_frame(self) -> pd.DataFrame:
-        oov_count = self.num_buckets or 1
-        meta = {
-            "kind": ["pad", "null", "oov", "unique"],
-            "offset": [PAD_OFFSET, NULL_OFFSET, OOV_OFFSET, OOV_OFFSET + oov_count],
-            "num_indices": [1, 1, oov_count, self.vocab.n_kept],
-        }
-        if self.has_sizes:
-            meta["num_observed"] = [0, self.vocab.null_size, self.vocab.oov_size, self.vocab.unique_size]
-        return pd.DataFrame(meta)
+    def _meta_columns(self):
+        """(name, dtype) of meta.<name>.parquet (categorify.py:801-822: kind = pad, null, oov,
+        unique; offset = PAD_OFFSET, NULL_OFFSET, OOV_OFFSET, first label; num_indices
+        [; num_observed]), for its pandas metadata"""
+        cols = [("kind", "object"), ("offset", np.int64), ("num_indices", np.int64)]
+        return cols + ([("num_observed", np.int64)] if self.has_sizes else [])
 
-    def write(self, base_path, force=False):
-        """categorify.py:731-822: unique.<name>.parquet (index = label) + meta.<name>.parquet."""
+    def _paths(self, base_path):
+        return ("/".join([str(base_path), f"meta.{self.name}.parquet"]),
+                "/".join([str(base_path), f"unique.{self.name}.parquet"]))
+
+    @property
+    def native_files(self) -> bool:
+        """int and float key spaces: both files are written by the library (engine.ArtifactWriter)"""
+        return isinstance(self.space, KeySpace) and self.space.kind in ("int", "float")
+
+    def write(self, base_path, force=False, writer=None):
+        """categorify.py:731-822: unique.<name>.parquet (index = label) + meta.<name>.parquet.
+        With `writer` (an engine.ArtifactWriter) the files of an int / float key space are only
+        queued; finish_write() completes them after writer.join()."""
         self.path = "/".join([str(base_path), f"unique.{self.name}.parquet"])
         if not force and _artifacts_lazy():
             self._written = False
             return self.path
         os.makedirs(base_path, exist_ok=True)
-        self._write_now(base_path, force)
+        if writer is not None and self.native_files:
+            self._submit(writer, base_path, force)
+        else:
+            self._write_now(base_path, force)
         return self.path
 
-    def _write_now(self, base_path, force):
-        import pyarrow as pa
-        import pyarrow.parquet as pq
-        meta_path = "/".join([str(base_path), f"meta.{self.name}.parquet"])
-        mf = self.meta_frame()
-        tb = pa.table({c: pa.array(mf[c].tolist() if c == "kind" else mf[c].to_numpy()) for c in mf.columns})
-        tb = tb.replace_schema_metadata({b"pandas": _pandas_meta(
-            [(c, "object" if c == "kind" else mf[c].dtype) for c in mf.columns], 0, len(mf))})
-        pq.write_table(tb, meta_path)
+    def _submit(self, writer, base_path, force):
+        """queue meta + unique files on the library's writer threads: no wait for the device here"""
+        meta_path, upath = self._paths(base_path)
+        key = self.key_names[0]
+        key_dtype = np.dtype(self.space.np_dtype or (np.int64 if self.space.kind == "int" else np.float64))
+        size_name = f"{self.name}_size" if self.has_sizes else None
+        head, tail = _pandas_meta_parts([(key, key_dtype)] + ([(size_name, np.int64)] if size_name else []),
+                                        self.index_start)
+        writer.submit_vocab(self.vocab, meta_path, _pandas_meta(self._meta_columns(), 0, 4), upath,
+                            -1 if force else EAGER_ARTIFACT_ROWS, key, key_dtype, size_name, self.index_start,
+                            self.num_buckets or 1, head, tail)
+        self._queued = (base_path, force)
+
+    def finish_write(self):
+        """after the ArtifactWriter of a write(..., writer=) joined: the file the library leaves to
+        pandas (an empty input's single null row) and the written flag"""
+        if self._queued is None:
+            return
+        base_path, force = self._queued
+        self._queued = None
         if force or self.vocab.n_kept <= EAGER_ARTIFACT_ROWS:
-            upath = "/".join([str(base_path), f"unique.{self.name}.parquet"])
-            plain = isinstance(self.space, KeySpace) and self.space.kind in ("int", "float") and self.vocab.n_total > 0
-            if plain:
-                k, sz = self._host_arrays()
-                arrays = {self.key_names[0]: np.asarray(self.space.decode(k))}
-                if self.has_sizes:
-                    arrays[f"{self.name}_size"] = sz
-                _write_numeric_parquet(upath, arrays, self.index_start)
-            else:
-                df = self.unique_frame()
-                if self.vocab.n_total == 0:   # categorify.py:1318-1324: empty input -> a single null row
-                    df = pd.DataFrame({n: pd.Series([None], dtype=object) for n in self.key_names})
-                df.to_parquet(upath, compression=None)
+            _, upath = self._paths(base_path)
+            if self.vocab.n_total == 0:
+                self._empty_unique_frame().to_parquet(upath, compression=None)
+            if self.path is None or os.path.abspath(upath) == os.path.abspath(self.path):
+                self._written = True
+
+    def _empty_unique_frame(self):
+        """categorify.py:1318-1324: empty input -> a single null row"""
+        return pd.DataFrame({n: pd.Series([None], dtype=object) for n in self.key_names})
+
+    def _write_now(self, base_path, force):
+        if self.native_files:
+            writer = engine.ArtifactWriter(1)
+            try:
+                self._submit(writer, base_path, force)
+            finally:
+                writer.join()
+            self.finish_write()
+            return
+        # string and combination key spaces: the meta file from the library, the vocabulary from pandas
+        meta_path, upath = self._paths(base_path)
+        v = self.vocab
+        engine.parquet_write_meta(meta_path, self.num_buckets or 1, v.n_kept, v.null_size, v.oov_size, v.unique_size,
+                                  self.has_sizes, _pandas_meta(self._meta_columns(), 0, 4))
+        if force or self.vocab.n_kept <= EAGER_ARTIFACT_ROWS:
+            df = self._empty_unique_frame() if self.vocab.n_total == 0 else self.unique_frame()
+            df.to_parquet(upath, compression=None)
             if self.path is None or os.path.abspath(upath) == os.path.abspath(self.path):
                 self._written = True
 
     def wait(self):
-        """kept for callers of the earlier threaded writer: writes are synchronous now"""
+        """kept for callers of the earlier threaded writer: writes are complete when write()
+        returns, or, with a writer, after its join() and finish_write()"""
         return None
 
     def ensure_written(self):
@@ -433,8 +452,8 @@ class Categorify(StatOperator):
                     flush()
             if world()[0] == 1:
                 # single GPU: every vocabulary is built straight from its handle — the small ones
-                # first, their keys / sizes on the way to pinned host memory (artefact files)
-                # before the builds of the sorted accumulators (large) are queued
+                # first, so that their artefact files can be written (fit_finalize) while the
+                # builds of the sorted accumulators (large) still run
                 return self._close_in_order(groups, state, {storage: "direct" for storage, _ in groups})
             from ..dist import global_merge_many, global_merge_sorted
             self._rows_bound_global = _global_rows(max(self._rows_seen.values(), default=0))
@@ -472,8 +491,6 @@ class Categorify(StatOperator):
         small = [g for g in groups if not large(g[0])]
         for storage, _ in small:
             fitted[storage] = self._close_group(storage, [storage], state[storage][0], state[storage][1], merged[storage])
-        for storage, _ in small:
-            fitted[storage].prefetch_host()
         for storage, _ in groups:
             if storage not in fitted:
                 fitted[storage] = self._close_group(storage, [storage], state[storage][0], state[storage][1],
@@ -582,15 +599,26 @@ class Categorify(StatOperator):
         idx_count = 0
         merged = dict(self.vocabs)
         merged.update(categories)
-        for name, fv in merged.items():
-            if self.single_table:                      # categorify.py:410-415, 1884-1897
-                fv.index_start = fv.index_start + idx_count
-                idx_count += fv.file_rows
-                fv._written = False
-            if name in categories or self.single_table:
-                fv.write(base)
-            self.categories[name] = fv.path
-            self.categories.fitted[name] = fv
+        # the int / float vocabularies' files are written by library threads, each as soon as its
+        # vocabulary is built; they are all joined here, so every eager file exists on return
+        writer = None
+        if not _artifacts_lazy() and any(fv.native_files for fv in merged.values()):
+            writer = engine.ArtifactWriter(WRITER_THREADS)
+        try:
+            for name, fv in merged.items():
+                if self.single_table:                      # categorify.py:410-415, 1884-1897
+                    fv.index_start = fv.index_start + idx_count
+                    idx_count += fv.file_rows
+                    fv._written = False
+                if name in categories or self.single_table:
+                    fv.write(base, writer=writer)
+                self.categories[name] = fv.path
+                self.categories.fitted[name] = fv
+        finally:
+            if writer is not None:
+                writer.join()
+        for fv in merged.values():
+            fv.finish_write()
 
     def clear(self):
         self.categories = _Categories()
