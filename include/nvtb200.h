@@ -508,6 +508,48 @@ int nvtb_gb_list_rows(const nvtb_col_t* leaves, const int64_t* lo, const int64_t
                       int64_t* off_out, void* out, uint8_t* out_valid, int64_t* total_host,
                       void* stream);
 
+/* ---- external-table join: JoinExternal operator (csrc/join.cu, K9) -------------------------
+ * Replaces, per partition, reference nvtabular/ops/join_external.py:148-164: df.merge(ext,
+ * left_on=on, right_on=on_ext, how=how) followed by sort_values("__tmp__") back to row order.
+ * Output rows follow left-row order, and the matches of one left row follow ext-table order.
+ *
+ * nvtb_join_create (join_external.py:148-164, the build side of the merge; once per operator):
+ * distinct_keys[n_groups] (int64) are the distinct valid ext keys, and run g of the ext rows in
+ * key order is ordered_rows[off[g] .. off[g + 1]) (off: n_groups + 1 int64), as the K8 calls
+ * nvtb_gb_order_codes / nvtb_gb_order_rows / nvtb_gb_segments leave them (stable: ext order
+ * within a key).  ordered_rows[null_lo .. null_hi) are the null-key ext rows, which null left
+ * keys join.  The handle copies off and ordered_rows and builds a wide table key -> run.
+ * n_ext < 2^31 (NVTB_EINVAL otherwise).  Synchronises. */
+typedef struct nvtb_join nvtb_join_t;
+int nvtb_join_create(nvtb_join_t** out, const int64_t* distinct_keys, int64_t n_groups,
+                     const int64_t* off, const int64_t* ordered_rows, int64_t n_ext,
+                     int64_t null_lo, int64_t null_hi, void* stream);
+/* n_groups and the largest run (null run included): 1 or less means every ext key is unique */
+int nvtb_join_info(const nvtb_join_t* j, int64_t* n_groups, int64_t* max_group);
+int nvtb_join_destroy(nvtb_join_t* j);
+/* Probe (join_external.py:148-164, the probe side of the merge): one pass over key (int32 or
+ * int64; a null row joins the null run).  how 0 = left, 1 = inner.
+ *   off_out == NULL: ext_row_out[i] = the ext row matching row i, or -1; *n_out_host = n.  This is
+ *     the whole join for a left join whose ext keys are unique.
+ *   otherwise: ext_row_out[i] = the position of row i's first match in key order, or -1, and
+ *     off_out[n + 1] (int64, 32-byte aligned) the exclusive scan of the rows each left row emits
+ *     (its match count; at least 1 in a left join); *n_out_host = off_out[n].  Synchronises. */
+int nvtb_join_probe(const nvtb_join_t* j, const nvtb_col_t* key, int64_t n, int how,
+                    int64_t* ext_row_out, int64_t* off_out, int64_t* n_out_host, void* stream);
+/* Expand (join_external.py:148-164, the rows the merge emits, already in left-row order): for
+ * every output row p < n_out, left_rows[p] = its left row and ext_rows[p] = its ext row (-1 for
+ * the unmatched row of a left join), from the probe's ext_row_first and off.  Balanced over
+ * output rows.  Outputs 32-byte aligned. */
+int nvtb_join_expand(const nvtb_join_t* j, const int64_t* ext_row_first, const int64_t* off,
+                     int64_t n, int64_t n_out, int64_t* left_rows, int64_t* ext_rows, void* stream);
+/* Gather (join_external.py:148-164, the merged columns): for k < ncols (<= 16) fixed-width
+ * columns, outs[k][p] = cols[k][rows[p]] for p < m, exact for every width (no fp64 round trip);
+ * rows[p] = -1 writes 0 and a null.  valids (NULL, or per column NULL or ceil(m/8) bitmask bytes)
+ * receive the output validity.  rows and the 4/8-byte outputs 32-byte aligned, 1-byte outputs
+ * 8-byte aligned. */
+int nvtb_join_gather(const nvtb_col_t* cols, int ncols, const int64_t* rows, int64_t m,
+                     void* const* outs, uint8_t* const* valids, void* stream);
+
 /* ---- cross-GPU collectives of the fit path (SURVEY.md 8e) ---------------------------------
  * nvtb_comm_t wraps an ncclComm_t: created here (rank 0 makes a unique id, the host runtime
  * hands it to every rank — torch.distributed broadcast, MPI, a file) or provided by the caller.

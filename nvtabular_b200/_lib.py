@@ -118,6 +118,12 @@ _SIGNATURES = {
     "nvtb_gb_reduce": (c_int, [POINTER(nvtb_col_t), c_void_p, c_int64, POINTER(c_void_p), POINTER(c_void_p), c_void_p]),
     "nvtb_gb_list_rows": (c_int, [POINTER(nvtb_col_t), c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
     "nvtb_gb_rank_stats": (c_int, [POINTER(nvtb_col_t), c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "nvtb_join_create": (c_int, [POINTER(c_void_p), c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
+    "nvtb_join_info": (c_int, [c_void_p, POINTER(c_int64), POINTER(c_int64)]),
+    "nvtb_join_destroy": (c_int, [c_void_p]),
+    "nvtb_join_probe": (c_int, [c_void_p, POINTER(nvtb_col_t), c_int64, c_int, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
+    "nvtb_join_expand": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
+    "nvtb_join_gather": (c_int, [POINTER(nvtb_col_t), c_int, c_void_p, c_int64, POINTER(c_void_p), POINTER(c_void_p), c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

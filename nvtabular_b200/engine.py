@@ -805,3 +805,84 @@ def gb_list_rows(leaves: Column, lo: torch.Tensor, hi: torch.Tensor) -> Column:
                                      byref(total), _lib.stream_ptr()))
     _count(2)
     return Column(out, valid, off, leaves.dictionary, None, leaves.is_bool)
+
+
+# ------------------------------------------------------------- external-table join (K9, csrc/join.cu)
+class JoinTable:
+    """The build side of JoinExternal on the device: ext rows in key order, the run of every
+    distinct key and a table key -> run (nvtb_join_create)."""
+
+    def __init__(self, distinct_keys: torch.Tensor, off: torch.Tensor, ordered_rows: torch.Tensor,
+                 null_lo: int, null_hi: int):
+        _lib.require_cuda()
+        self.lib = _lib.load()
+        self.h = c_void_p()
+        keys = distinct_keys.to(torch.int64).contiguous()
+        rows = ordered_rows.to(torch.int64).contiguous()
+        _lib.check(self.lib.nvtb_join_create(byref(self.h), _ptr(keys), keys.numel(), _ptr(off), _ptr(rows),
+                                             rows.numel(), int(null_lo), int(null_hi), _lib.stream_ptr()))
+        _count(2)
+        g, mx = c_int64(0), c_int64(0)
+        _lib.check(self.lib.nvtb_join_info(self.h, byref(g), byref(mx)))
+        self.n_groups, self.max_group = g.value, mx.value
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None) is not None and self.h.value:
+                self.lib.nvtb_join_destroy(self.h)
+                self.h = c_void_p()
+        except Exception:
+            pass
+
+    def probe(self, key: Column, how: str, scan: bool):
+        """-> (ext int64[n], off int64[n + 1] | None, n_out).  Without `scan`: the ext row of every
+        left row (-1 = no match).  With it: the first match's position in key order and the output
+        offsets (nvtb_join_probe; one host read)."""
+        n = key.data.numel()
+        dev = key.data.device
+        ext = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+        off = torch.empty(n + 1, dtype=torch.int64, device=dev) if scan else None
+        n_out = c_int64(0)
+        with _timed("join_probe", _in_bytes([key]) + n * (16.0 if scan else 8.0)):
+            _lib.check(self.lib.nvtb_join_probe(self.h, _descs([key]), n, 0 if how == "left" else 1, _ptr(ext),
+                                                _ptr(off), byref(n_out), _lib.stream_ptr()))
+        _count(4 if scan else 1)
+        return ext[:n], off, n_out.value
+
+    def expand(self, first: torch.Tensor, off: torch.Tensor, n_out: int):
+        """-> (left rows, ext rows) int64[n_out] of every output row (nvtb_join_expand)"""
+        dev = first.device
+        left = torch.empty(max(n_out, 1), dtype=torch.int64, device=dev)
+        ext = torch.empty(max(n_out, 1), dtype=torch.int64, device=dev)
+        with _timed("join_expand", n_out * 16.0 + first.numel() * 8.0):
+            _lib.check(self.lib.nvtb_join_expand(self.h, _ptr(first), _ptr(off), first.numel(), n_out, _ptr(left),
+                                                 _ptr(ext), _lib.stream_ptr()))
+        _count()
+        return left[:n_out], ext[:n_out]
+
+
+JOIN_GATHER_MAX_COLS = 16   # columns of one nvtb_join_gather launch (kMaxJoinCols, csrc/join.cu)
+
+
+def join_gather(cols: Sequence[Column], rows: torch.Tensor, masked: Sequence[bool]) -> List[Column]:
+    """flat columns at int64 `rows` (-1 = null) -> Columns with the sources' dtype, dictionary and
+    bool flag; output k gets a validity bitmask when masked[k] or its source has one
+    (nvtb_join_gather)"""
+    lib = _lib.load()
+    m = rows.numel()
+    dev = rows.device
+    # an empty source (an empty ext table) is only ever read at row -1: give the kernel one row
+    cols = [c if c.data.numel() else Column(torch.zeros(1, dtype=c.data.dtype, device=dev), None, None,
+                                            c.dictionary, None, c.is_bool) for c in cols]
+    outs = [torch.empty(max(m, 1), dtype=c.data.dtype, device=dev) for c in cols]
+    valids = [_bitmask(m, dev) if (mk or c.validity is not None) else None for c, mk in zip(cols, masked)]
+    for s in range(0, len(cols), JOIN_GATHER_MAX_COLS):
+        e = s + JOIN_GATHER_MAX_COLS
+        nbytes = m * 8.0 + sum(m * (c.data.element_size() + 0.125) for c in cols[s:e])
+        with _timed("join_gather", nbytes):
+            _lib.check(lib.nvtb_join_gather(_descs(cols[s:e]), len(cols[s:e]), _ptr(rows), m,
+                                            _lib.ptr_array([o.data_ptr() for o in outs[s:e]]),
+                                            _lib.ptr_array([v.data_ptr() if v is not None else None
+                                                            for v in valids[s:e]]), _lib.stream_ptr()))
+        _count()
+    return [Column(o[:m], v, None, c.dictionary, None, c.is_bool) for o, v, c in zip(outs, valids, cols)]

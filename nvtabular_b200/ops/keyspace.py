@@ -217,11 +217,13 @@ class ComboKeySpace:
         return len(cols) == 2 and all((not c.is_string) and c.data.dtype == torch.int32 for c in cols)
 
     @classmethod
-    def fit(cls, partitions: Sequence[Sequence[Column]], ncomp: Optional[int] = None) -> "ComboKeySpace":
+    def fit(cls, partitions: Sequence[Sequence[Column]], ncomp: Optional[int] = None,
+            sync: bool = True) -> "ComboKeySpace":
         """partitions: per partition, the component columns (leaves).  `ncomp` must be given
-        when a rank may hold no partition (every rank runs the same collectives)."""
+        when a rank may hold no partition (every rank runs the same collectives).  `sync=False`
+        builds a rank-local space and runs no collective (a table every rank holds whole)."""
         ncomp = ncomp if ncomp is not None else len(partitions[0])
-        spaces = [KeySpace.for_columns([p[j] for p in partitions]) for j in range(ncomp)]
+        spaces = [KeySpace.for_columns([p[j] for p in partitions], sync=sync) for j in range(ncomp)]
         # decided from the (rank-synchronised) spaces, so every rank takes the same path
         if ncomp == 2 and all(s.kind == "int" and s.np_dtype == np.dtype("int32") for s in spaces) and \
                 all(cls.can_pack_direct(p) for p in partitions):
@@ -231,7 +233,7 @@ class ComboKeySpace:
         running = None
         for j in range(ncomp):
             comp_keys = [spaces[j].keys_for(p[j]) for p in partitions]
-            vocab, host = cls._rank_vocab(comp_keys)
+            vocab, host = cls._rank_vocab(comp_keys, sync)
             self.rank_vocabs.append(vocab)
             self.rank_keys.append(host)
             ranks = [cls._rank(vocab, k) for k in comp_keys]
@@ -240,19 +242,20 @@ class ComboKeySpace:
             else:
                 packed = [engine.pack_keys2(a, b) for a, b in zip(running, ranks)]
                 if j < ncomp - 1:
-                    pv, ph = cls._rank_vocab(packed)
+                    pv, ph = cls._rank_vocab(packed, sync)
                     self.rank_vocabs.append(pv)
                     self.rank_keys.append(ph)
                     running = [cls._rank(pv, k) for k in packed]
         return self
 
     @staticmethod
-    def _rank_vocab(key_cols: Sequence[Column]):
+    def _rank_vocab(key_cols: Sequence[Column], sync: bool = True):
         from ..dist import global_merge
         agg = engine.HashAgg(0)
         for k in key_cols:
             agg.insert(k)
-        keys, _, _, _, _ = global_merge(agg)     # identical on every rank (single GPU: an export)
+        # identical on every rank (single GPU, or sync=False: an export)
+        keys, _, _, _, _ = global_merge(agg) if sync else agg.export()
         keys, _ = torch.sort(keys)
         return engine.Vocab.from_arrays(keys), keys.cpu().numpy()
 

@@ -150,3 +150,21 @@ def session_frame(rows: int, seed: int = 1234, device="cuda", mean_length: float
     price = torch.rand(rows, generator=g, device=device, dtype=torch.float32) * 100
     return DeviceFrame({"session_id": Column(sid), "item_id": Column(item), "ts": Column(ts),
                         "price": Column(price)}), n_sess
+
+
+GENRES = ["Action", "Adventure", "Animation", "Children", "Comedy", "Crime", "Documentary", "Drama", "Fantasy",
+          "Film-Noir", "Horror", "IMAX", "Musical", "Mystery", "Romance", "Sci-Fi", "Thriller", "War"]
+
+
+def movies_frame(n_movies: int = 60_000, seed: int = 8765, device="cuda") -> DeviceFrame:
+    """MovieLens-shaped movies table for the ratings of movielens_frame: movieId = the same scattered
+    ids (scatter_ids(1..n_movies)), genres = a list of 1-6 of 18 genre names, year int32."""
+    g = _gen(seed, device)
+    ids = scatter_ids(torch.arange(1, n_movies + 1, device=device, dtype=torch.int64))
+    lens = torch.randint(1, 7, (n_movies,), generator=g, device=device, dtype=torch.int64)
+    off = torch.zeros(n_movies + 1, dtype=torch.int64, device=device)
+    off[1:] = torch.cumsum(lens, 0)
+    codes = torch.randint(0, len(GENRES), (int(off[-1].item()),), generator=g, device=device, dtype=torch.int32)
+    year = torch.randint(1900, 2020, (n_movies,), generator=g, device=device, dtype=torch.int32)
+    return DeviceFrame({"movieId": Column(ids), "genres": Column(codes, None, off, np.array(sorted(GENRES), dtype=object)),
+                        "year": Column(year)})
