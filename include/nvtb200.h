@@ -501,12 +501,45 @@ int nvtb_gb_rank_stats(const nvtb_col_t* col, const uint64_t* codes, const uint8
                        int64_t n_groups, float* median_out, int32_t* nunique_out, void* stream);
 
 /* Sub-lists [lo[g], hi[g]) of a list column's leaves, concatenated (first / last of a list input
- * column, reference test_groupby_list_first_last).  Called twice: with out == NULL it writes
- * off_out[m + 1] and *total_host (synchronises); then with out (total_host leaves of the leaf
- * dtype) and out_valid (NULL, or a zeroed 4-byte-aligned bitmask) it copies the leaves. */
+ * column, reference test_groupby_list_first_last; the unpadded ListSlice).  Called twice: with
+ * out == NULL it writes off_out[m + 1] and *total_host (a multi-CTA scan; synchronises); then with
+ * out (total_host leaves of the leaf dtype) and out_valid (NULL, or ceil(total_host / 8) bitmask
+ * bytes, which it overwrites) it copies the leaves, balanced over output elements. */
 int nvtb_gb_list_rows(const nvtb_col_t* leaves, const int64_t* lo, const int64_t* hi, int64_t m,
                       int64_t* off_out, void* out, uint8_t* out_valid, int64_t* total_host,
                       void* stream);
+
+/* ---- session operators: ListSlice and DifferenceLag (csrc/session.cu, K10) -----------------
+ * nvtb_list_slice_bounds (reference nvtabular/ops/list_slice.py:78-144 and its GPU kernel
+ * _calculate_row_sizes, list_slice.py:180-198): for every row i of a list column with offsets[n + 1],
+ * [lo_out[i], hi_out[i]) is the absolute leaf range of Python's row[start:end]: a negative index
+ * counts from the row end, both ends are clamped to [0, len] and hi >= lo.  nvtb_gb_list_rows over
+ * these bounds is the unpadded slice. */
+int nvtb_list_slice_bounds(const int64_t* offsets, int64_t n, int64_t start, int64_t end,
+                           int64_t* lo_out, int64_t* hi_out, void* stream);
+/* nvtb_list_slice_pad (list_slice.py:78-144 with pad=True, and _slice_rows, list_slice.py:201-228):
+ * the dense n x L slice: out[i * L + k] = row i's k-th element of row[start:end] for k below its
+ * length, else the pad value (pad_bits: the value's bit pattern in the leaf dtype, low bytes),
+ * which is valid.  Copied elements carry the leaf validity (out_valid: NULL when the leaves have
+ * none, else ceil(n * L / 8) bytes).  off_out[n + 1] = i * L.  out 32-byte aligned (1-byte
+ * leaves: 8-byte).  No scan and no host read. */
+int nvtb_list_slice_pad(const nvtb_col_t* leaves, const int64_t* offsets, int64_t n, int64_t start,
+                        int64_t end, int64_t L, uint64_t pad_bits, void* out, uint8_t* out_valid,
+                        int64_t* off_out, void* stream);
+/* nvtb_lag_same_key (reference nvtabular/ops/difference_lag.py:65-75, the partition mask): bit i of
+ * same_out (ceil(n/8) bytes) is set when 0 <= i - shift < n and every one of the n_keys (<= 8) key
+ * columns is valid and equal at i and i - shift.  Floats compare with IEEE == (-0.0 == +0.0, NaN
+ * equals nothing); integers, uint8 and string codes compare by value. */
+int nvtb_lag_same_key(const nvtb_col_t* keys, int n_keys, int64_t n, int64_t shift, uint8_t* same_out,
+                      void* stream);
+/* nvtb_difference_lag (difference_lag.py:76-80): for k < ncols (<= 16) value columns (int32, int64,
+ * uint8, float32, float64), outs[k][i] = x[i] - x[i - shift] as float32 where bit i of `same`
+ * (nvtb_lag_same_key with the same n and shift) is set and both values are valid; otherwise 0 and
+ * a cleared bit of out_valids[k] (ceil(n/8) bytes each).  Integers subtract in int64 (wrapping)
+ * and round once; float32 subtracts in float32; float64 in float64, then rounds once.  Outputs
+ * 32-byte aligned. */
+int nvtb_difference_lag(const nvtb_col_t* cols, int ncols, int64_t n, int64_t shift, const uint8_t* same,
+                        float* const* outs, uint8_t* const* out_valids, void* stream);
 
 /* ---- external-table join: JoinExternal operator (csrc/join.cu, K9) -------------------------
  * Replaces, per partition, reference nvtabular/ops/join_external.py:148-164: df.merge(ext,

@@ -124,6 +124,12 @@ _SIGNATURES = {
     "nvtb_join_probe": (c_int, [c_void_p, POINTER(nvtb_col_t), c_int64, c_int, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
     "nvtb_join_expand": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "nvtb_join_gather": (c_int, [POINTER(nvtb_col_t), c_int, c_void_p, c_int64, POINTER(c_void_p), POINTER(c_void_p), c_void_p]),
+    "nvtb_list_slice_bounds": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
+    "nvtb_list_slice_pad": (c_int, [POINTER(nvtb_col_t), c_void_p, c_int64, c_int64, c_int64, c_int64, c_uint64, c_void_p,
+                                    c_void_p, c_void_p, c_void_p]),
+    "nvtb_lag_same_key": (c_int, [POINTER(nvtb_col_t), c_int, c_int64, c_int64, c_void_p, c_void_p]),
+    "nvtb_difference_lag": (c_int, [POINTER(nvtb_col_t), c_int, c_int64, c_int64, c_void_p, POINTER(c_void_p),
+                                    POINTER(c_void_p), c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -21,6 +21,7 @@
 // No floating-point atomics anywhere: outputs are bit-identical from run to run.
 #include "common.cuh"
 #include "radix.cuh"
+#include "scan.cuh"
 
 namespace nvtb {
 namespace {
@@ -528,39 +529,56 @@ rank_stats_kernel(const T* __restrict__ d, const uint64_t* __restrict__ codes, c
 }
 
 // ---------------------------------------------------------------------------------------
-// sub-lists of a list column (first / last of a list input): off[g] = sum of (hi - lo) before g
+// sub-lists of a list column (first / last of a list input, ListSlice): output row g holds
+// leaves[lo[g], hi[g]).  Its offsets are the exclusive scan (scan.cuh) of the lengths.
 // ---------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024)
-list_offsets_kernel(const int64_t* __restrict__ lo, const int64_t* __restrict__ hi, int64_t m,
-                    int64_t* __restrict__ off, unsigned long long* __restrict__ total) {
-  __shared__ uint32_t ws[1024 / 32 + 1];
-  int64_t carry = 0;
-  for (int64_t c0 = 0; c0 < m; c0 += 1024) {
-    const int64_t i = c0 + threadIdx.x;
-    const int64_t len = i < m ? hi[i] - lo[i] : 0;
-    // lengths are split into two 32-bit halves so that the 32-bit block scan carries them exactly
-    uint32_t t_lo, t_hi;
-    const uint32_t e_lo = block_excl_scan_u32<1024>((uint32_t)(len & 0xFFFFFFFF), ws, &t_lo);
-    const uint32_t e_hi = block_excl_scan_u32<1024>((uint32_t)(len >> 32), ws, &t_hi);
-    if (i < m) off[i] = carry + (int64_t)e_lo + ((int64_t)e_hi << 32);
-    carry += (int64_t)t_lo + ((int64_t)t_hi << 32);
-  }
-  if (threadIdx.x == 0) { off[m] = carry; *total = (unsigned long long)carry; }
+__global__ void __launch_bounds__(kGbThreads)
+list_lengths_kernel(const int64_t* __restrict__ lo, const int64_t* __restrict__ hi, int64_t m,
+                    int64_t* __restrict__ len) {
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < m; g += (int64_t)gridDim.x * blockDim.x)
+    len[g] = __ldg(hi + g) - __ldg(lo + g);
 }
 
-// warp per sub-list: out[off[g] + k] = src[lo[g] + k]; validity bits are ORed into 32-bit words
+// last g in [a, b) with off[g] <= p (off[a] <= p is given)
+__device__ __forceinline__ int64_t last_at_or_below(const int64_t* __restrict__ off, int64_t a, int64_t b, int64_t p) {
+  while (b - a > 1) {
+    const int64_t mid = (a + b) >> 1;
+    if (__ldg(off + mid) <= p) a = mid; else b = mid;
+  }
+  return a;
+}
+
+// Balanced over OUTPUT positions: every lane owns 8 consecutive ones (one validity byte, so no
+// atomics) and finds the sub-list of each by binary search over off, inside the bracket of its
+// first and last position's sub-lists.  A table of 10^7 short lists keeps every lane busy.
 template <typename T>
 __global__ void __launch_bounds__(kGbThreads)
 list_copy_kernel(const T* __restrict__ src, const uint8_t* __restrict__ src_valid, const int64_t* __restrict__ lo,
-                 const int64_t* __restrict__ off, int64_t m, T* __restrict__ out, uint32_t* __restrict__ out_valid) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warps = (int64_t)gridDim.x * (blockDim.x / 32);
-  for (int64_t g = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < m; g += warps) {
-    const int64_t s = lo[g], d = off[g], len = off[g + 1] - off[g];
-    for (int64_t k = lane; k < len; k += 32) {
-      out[d + k] = src[s + k];
-      if (out_valid != nullptr && bit_at(src_valid, s + k)) atomicOr(out_valid + ((d + k) >> 5), 1u << ((d + k) & 31));
+                 const int64_t* __restrict__ off, int64_t m, int64_t total, bool aligned, T* __restrict__ out,
+                 uint8_t* __restrict__ out_valid) {
+  const int64_t nchunks = (total + 7) / 8;
+  for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nchunks; c += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p0 = c * 8;
+    const int64_t pe = p0 + 7 < total ? p0 + 7 : total - 1;
+    const int64_t g0 = last_at_or_below(off, 0, m, p0);
+    const int64_t g1 = last_at_or_below(off, g0, m, pe);
+    T v[8];
+    unsigned vb = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int64_t p = p0 + k <= pe ? p0 + k : pe;
+      const int64_t g = last_at_or_below(off, g0, g1 + 1, p);
+      const int64_t s = __ldg(lo + g) + (p - __ldg(off + g));
+      v[k] = src[s];
+      if (p0 + k <= pe && bit_at(src_valid, s)) vb |= 1u << k;
     }
+    if (aligned && p0 + 8 <= total) {
+      st_rows8<T>(out + p0, v);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) if (p0 + k < total) out[p0 + k] = v[k];
+    }
+    if (out_valid != nullptr) out_valid[p0 >> 3] = (uint8_t)vb;
   }
 }
 
@@ -789,29 +807,32 @@ int nvtb_gb_list_rows(const nvtb_col_t* leaves, const int64_t* lo, const int64_t
   cudaStream_t st = (cudaStream_t)stream;
   if (out == nullptr) {
     *total_host = 0;
-    unsigned long long* t = nullptr;
-    NVTB_CUDA_OK(cudaMallocAsync(&t, sizeof(unsigned long long), st));
-    NVTB_CUDA_OK(cudaMemsetAsync(t, 0, sizeof(unsigned long long), st));
-    NVTB_CUDA_OK(cudaMemsetAsync(off_out, 0, sizeof(int64_t), st));
+    NVTB_REQUIRE(m == 0 || (lo && hi), "NULL bounds");
+    // the scan needs 32-byte aligned offsets: scan in a scratch copy when off_out is not
+    const bool aligned = is_aligned32(off_out);
+    int64_t* buf = off_out;
+    if (!aligned) NVTB_CUDA_OK(cudaMallocAsync(&buf, sizeof(int64_t) * (m + 1), st));
     if (m > 0) {
-      NVTB_REQUIRE(lo && hi, "NULL bounds");
-      list_offsets_kernel<<<1, 1024, 0, st>>>(lo, hi, m, off_out, t);
+      list_lengths_kernel<<<grid_for(m, kGbThreads), kGbThreads, 0, st>>>(lo, hi, m, buf);
       NVTB_LAUNCH_OK();
     }
-    unsigned long long h = 0;
-    NVTB_CUDA_OK(cudaMemcpyAsync(&h, t, sizeof(h), cudaMemcpyDeviceToHost, st));
-    NVTB_CUDA_OK(cudaFreeAsync(t, st));
-    NVTB_CUDA_OK(cudaStreamSynchronize(st));
-    *total_host = (int64_t)h;
-    return NVTB_OK;
+    const int rc = excl_scan_i64(buf, m, total_host, st);
+    if (!aligned) {
+      NVTB_CUDA_OK(cudaMemcpyAsync(off_out, buf, sizeof(int64_t) * (m + 1), cudaMemcpyDeviceToDevice, st));
+      NVTB_CUDA_OK(cudaFreeAsync(buf, st));
+      NVTB_CUDA_OK(cudaStreamSynchronize(st));
+    }
+    return rc;
   }
-  if (m == 0 || *total_host == 0) return NVTB_OK;
-  const int grid = grid_for(m, kGbThreads / 32);
-  uint32_t* ov = reinterpret_cast<uint32_t*>(out_valid);
+  const int64_t total = *total_host;
+  if (m == 0 || total == 0) return NVTB_OK;
+  NVTB_REQUIRE(leaves->data && lo, "NULL leaves / bounds");
+  const int grid = grid_for((total + 7) / 8, kGbThreads);
+  const uintptr_t a = reinterpret_cast<uintptr_t>(out);
   switch (dtype_size(leaves->dtype)) {
-    case 1: list_copy_kernel<uint8_t><<<grid, kGbThreads, 0, st>>>((const uint8_t*)leaves->data, leaves->validity, lo, off_out, m, (uint8_t*)out, ov); break;
-    case 4: list_copy_kernel<uint32_t><<<grid, kGbThreads, 0, st>>>((const uint32_t*)leaves->data, leaves->validity, lo, off_out, m, (uint32_t*)out, ov); break;
-    case 8: list_copy_kernel<uint64_t><<<grid, kGbThreads, 0, st>>>((const uint64_t*)leaves->data, leaves->validity, lo, off_out, m, (uint64_t*)out, ov); break;
+    case 1: list_copy_kernel<uint8_t><<<grid, kGbThreads, 0, st>>>((const uint8_t*)leaves->data, leaves->validity, lo, off_out, m, total, (a & 7u) == 0, (uint8_t*)out, out_valid); break;
+    case 4: list_copy_kernel<uint32_t><<<grid, kGbThreads, 0, st>>>((const uint32_t*)leaves->data, leaves->validity, lo, off_out, m, total, (a & 31u) == 0, (uint32_t*)out, out_valid); break;
+    case 8: list_copy_kernel<uint64_t><<<grid, kGbThreads, 0, st>>>((const uint64_t*)leaves->data, leaves->validity, lo, off_out, m, total, (a & 31u) == 0, (uint64_t*)out, out_valid); break;
     default: set_error("nvtb_gb_list_rows: unsupported dtype %d", (int)leaves->dtype); return NVTB_EINVAL;
   }
   NVTB_LAUNCH_OK();

@@ -25,8 +25,6 @@ namespace nvtb {
 namespace {
 
 constexpr int kJoinThreads = 256;
-constexpr int kJoinTile = kJoinThreads * kRows;        // 2048 rows per scan tile: 8 per lane
-constexpr int kScanThreads = 1024;
 constexpr int kMaxJoinCols = 16;
 
 struct JoinCols {
@@ -77,6 +75,16 @@ join_table_build_kernel(const int64_t* __restrict__ keys, const int64_t* __restr
   if ((threadIdx.x & 31) == 0 && longest) atomicMax(scal + 1, longest);
 }
 
+}  // namespace
+}  // namespace nvtb
+
+// Included after the build kernels, not at the top: the kernels are then emitted in the same
+// order as when the scan lived in this file, and the file's SASS is byte-identical to that.
+#include "scan.cuh"
+
+namespace nvtb {
+namespace {
+
 // ---------------------------------------------------------------------------------------
 // probe
 // ---------------------------------------------------------------------------------------
@@ -107,104 +115,6 @@ join_probe_kernel(const K* __restrict__ keys, const uint8_t* __restrict__ mask, 
     } else {
       ext_out[i] = pos >= 0 ? __ldg(rows + pos) : -1;
     }
-  }
-}
-
-// ---- exclusive scan of the int64 emit counts, in place: tile sums, one-CTA scan, tile apply ----
-template <int T>
-__device__ __forceinline__ long long block_excl_scan_i64(long long v, long long* ws /*[T/32 + 1]*/, long long* total) {
-  long long incl = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-    if ((threadIdx.x & 31) >= o) incl += y;
-  }
-  if ((threadIdx.x & 31) == 31) ws[threadIdx.x >> 5] = incl;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    const long long w = threadIdx.x < T / 32 ? ws[threadIdx.x] : 0;
-    long long wi = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const long long y = __shfl_up_sync(0xFFFFFFFFu, wi, o);
-      if (threadIdx.x >= o) wi += y;
-    }
-    if (threadIdx.x < T / 32) ws[threadIdx.x] = wi - w;
-    if (threadIdx.x == T / 32 - 1) ws[T / 32] = wi;
-  }
-  __syncthreads();
-  const long long out = ws[threadIdx.x >> 5] + incl - v;
-  *total = ws[T / 32];
-  __syncthreads();
-  return out;
-}
-
-__device__ __forceinline__ void load8_i64(const int64_t* __restrict__ p, int64_t i, int64_t n, int64_t (&v)[8]) {
-  if (i + 8 <= n) {
-    ld_rows8<int64_t>(p + i, v);
-  } else {
-#pragma unroll
-    for (int k = 0; k < 8; ++k) v[k] = i + k < n ? p[i + k] : 0;
-  }
-}
-
-__global__ void __launch_bounds__(kJoinThreads)
-join_tile_sums_kernel(const int64_t* __restrict__ counts, int64_t n, long long* __restrict__ tile_sum) {
-  __shared__ long long ws[kJoinThreads / 32 + 1];
-  const int64_t i = (int64_t)blockIdx.x * kJoinTile + (int64_t)threadIdx.x * 8;
-  int64_t v[8];
-  long long s = 0;
-  if (i < n) {
-    load8_i64(counts, i, n, v);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) s += v[k];
-  }
-  long long tot;
-  block_excl_scan_i64<kJoinThreads>(s, ws, &tot);
-  if (threadIdx.x == 0) tile_sum[blockIdx.x] = tot;
-}
-
-__global__ void __launch_bounds__(kScanThreads)
-join_tile_scan_kernel(long long* __restrict__ tile, int64_t ntiles, int64_t* __restrict__ off_end,
-                      unsigned long long* __restrict__ total) {
-  __shared__ long long ws[kScanThreads / 32 + 1];
-  long long carry = 0;
-  for (int64_t c0 = 0; c0 < ntiles; c0 += kScanThreads) {
-    const int64_t i = c0 + threadIdx.x;
-    const long long v = i < ntiles ? tile[i] : 0;
-    long long tot;
-    const long long ex = block_excl_scan_i64<kScanThreads>(v, ws, &tot);
-    if (i < ntiles) tile[i] = carry + ex;
-    carry += tot;
-  }
-  if (threadIdx.x == 0) { *off_end = carry; *total = (unsigned long long)carry; }
-}
-
-__global__ void __launch_bounds__(kJoinThreads)
-join_tile_apply_kernel(int64_t* __restrict__ off, int64_t n, const long long* __restrict__ tile_base) {
-  __shared__ long long ws[kJoinThreads / 32 + 1];
-  const int64_t i = (int64_t)blockIdx.x * kJoinTile + (int64_t)threadIdx.x * 8;
-  int64_t v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  long long s = 0;
-  if (i < n) {
-    load8_i64(off, i, n, v);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) s += v[k];
-  }
-  long long tot;
-  long long run = tile_base[blockIdx.x] + block_excl_scan_i64<kJoinThreads>(s, ws, &tot);
-  if (i >= n) return;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const long long c = v[k];
-    v[k] = run;
-    run += c;
-  }
-  if (i + 8 <= n) {
-    st_rows8<int64_t>(off + i, v);
-  } else {
-#pragma unroll
-    for (int k = 0; k < 8; ++k) if (i + k < n) off[i + k] = v[k];
   }
 }
 
@@ -404,26 +314,7 @@ int nvtb_join_probe(const nvtb_join_t* j, const nvtb_col_t* key, int64_t n, int 
     NVTB_LAUNCH_OK();
   }
   if (off_out == nullptr) return NVTB_OK;
-  const int64_t ntiles = (n + kJoinTile - 1) / kJoinTile;
-  long long* tiles = nullptr;
-  NVTB_CUDA_OK(cudaMallocAsync(&tiles, sizeof(long long) * (ntiles + 1), st));
-  unsigned long long* total = reinterpret_cast<unsigned long long*>(tiles + ntiles);
-  if (ntiles > 0) {
-    join_tile_sums_kernel<<<(unsigned)ntiles, kJoinThreads, 0, st>>>(off_out, n, tiles);
-    NVTB_LAUNCH_OK();
-  }
-  join_tile_scan_kernel<<<1, kScanThreads, 0, st>>>(tiles, ntiles, off_out + n, total);
-  NVTB_LAUNCH_OK();
-  if (ntiles > 0) {
-    join_tile_apply_kernel<<<(unsigned)ntiles, kJoinThreads, 0, st>>>(off_out, n, tiles);
-    NVTB_LAUNCH_OK();
-  }
-  unsigned long long h = 0;
-  NVTB_CUDA_OK(cudaMemcpyAsync(&h, total, sizeof(h), cudaMemcpyDeviceToHost, st));
-  NVTB_CUDA_OK(cudaFreeAsync(tiles, st));
-  NVTB_CUDA_OK(cudaStreamSynchronize(st));
-  *n_out_host = (int64_t)h;
-  return NVTB_OK;
+  return excl_scan_i64(off_out, n, n_out_host, st);
 }
 
 int nvtb_join_expand(const nvtb_join_t* j, const int64_t* ext_row_first, const int64_t* off, int64_t n, int64_t n_out,

@@ -807,6 +807,78 @@ def gb_list_rows(leaves: Column, lo: torch.Tensor, hi: torch.Tensor) -> Column:
     return Column(out, valid, off, leaves.dictionary, None, leaves.is_bool)
 
 
+# ------------------------------------------------------------- session operators (K10, csrc/session.cu)
+LAG_MAX_KEYS = 8    # partition columns of one nvtb_lag_same_key launch (kMaxLagKeys, csrc/session.cu)
+LAG_MAX_COLS = 16   # value columns of one nvtb_difference_lag launch (kMaxLagCols)
+
+
+def list_slice(col: Column, start: int, end: int) -> Column:
+    """row[start:end] of every row of a list column: the leaf bounds (nvtb_list_slice_bounds), then
+    the sub-list copy (nvtb_gb_list_rows).  The input is only read."""
+    lib = _lib.load()
+    n = col.nrows
+    dev = col.data.device
+    lo = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+    hi = torch.empty(max(n, 1), dtype=torch.int64, device=dev)
+    with _timed("list_slice_bounds", n * 24.0):
+        _lib.check(lib.nvtb_list_slice_bounds(_ptr(col.offsets), n, int(start), int(end), _ptr(lo), _ptr(hi),
+                                              _lib.stream_ptr()))
+    _count()
+    return gb_list_rows(col.leaves(), lo[:n], hi[:n])
+
+
+def list_slice_pad(col: Column, start: int, end: int, width: int, pad_bits: int) -> Column:
+    """the dense n x width slice of a list column, padded with the value whose bit pattern in the
+    leaf dtype is pad_bits (nvtb_list_slice_pad)"""
+    lib = _lib.load()
+    leaves = col.leaves()
+    n = col.nrows
+    m = n * width
+    dev = col.data.device
+    out = torch.empty(max(m, 1), dtype=leaves.data.dtype, device=dev)
+    valid = _bitmask(m, dev) if leaves.validity is not None else None
+    off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    with _timed("list_slice_pad", n * 16.0 + m * (leaves.data.element_size() * 2.0 + 0.25)):
+        _lib.check(lib.nvtb_list_slice_pad(_descs([leaves]), _ptr(col.offsets), n, int(start), int(end), int(width),
+                                           int(pad_bits), _ptr(out), _ptr(valid), _ptr(off), _lib.stream_ptr()))
+    _count()
+    return Column(out[:m], valid, off, leaves.dictionary, None, leaves.is_bool)
+
+
+def lag_same_key(keys: Sequence[Column], n: int, shift: int) -> torch.Tensor:
+    """bitmask: bit i set when row i - shift is in the frame and every key is valid and equal at i
+    and i - shift (nvtb_lag_same_key)"""
+    lib = _lib.load()
+    if len(keys) > LAG_MAX_KEYS:
+        raise ValueError(f"at most {LAG_MAX_KEYS} partition columns, got {len(keys)}")
+    same = _bitmask(n, keys[0].data.device)
+    shift = max(-n, min(n, int(shift)))
+    with _timed("lag_same_key", _in_bytes(keys) + n / 8.0):
+        _lib.check(lib.nvtb_lag_same_key(_descs(keys), len(keys), n, shift, _ptr(same), _lib.stream_ptr()))
+    _count()
+    return same
+
+
+def difference_lag(cols: Sequence[Column], same: torch.Tensor, shift: int) -> List[Column]:
+    """float32 x[i] - x[i - shift] of every column where `same` (lag_same_key with this shift) has
+    bit i and both values are valid, else null (nvtb_difference_lag)"""
+    lib = _lib.load()
+    n = _check_same_len(cols)
+    dev = cols[0].data.device
+    shift = max(-n, min(n, int(shift)))
+    outs = [torch.empty(max(n, 1), dtype=torch.float32, device=dev) for _ in cols]
+    valids = [_bitmask(n, dev) for _ in cols]
+    for s in range(0, len(cols), LAG_MAX_COLS):
+        e = s + LAG_MAX_COLS
+        with _timed("difference_lag", _in_bytes(cols[s:e]) + n * (4.125 * len(cols[s:e]) + 0.125)):
+            _lib.check(lib.nvtb_difference_lag(_descs(cols[s:e]), len(cols[s:e]), n, shift, _ptr(same),
+                                               _lib.ptr_array([o.data_ptr() for o in outs[s:e]]),
+                                               _lib.ptr_array([v.data_ptr() for v in valids[s:e]]),
+                                               _lib.stream_ptr()))
+        _count()
+    return [Column(o[:n], v) for o, v in zip(outs, valids)]
+
+
 # ------------------------------------------------------------- external-table join (K9, csrc/join.cu)
 class JoinTable:
     """The build side of JoinExternal on the device: ext rows in key order, the run of every

@@ -247,6 +247,11 @@ def _registry():
             lambda p, s, adir: ops.Groupby(groupby_cols=p.get("groupby_cols"), sort_cols=p.get("sort_cols"),
                                            aggs=p.get("aggs", "list"), name_sep=p.get("name_sep", "_"),
                                            ascending=p.get("ascending", True))),
+        "nvtabular.ops.list_slice.ListSlice": (
+            ops.ListSlice, lambda op, adir: ({"start": op.start, "end": op.end, "pad": op.pad,
+                                              "pad_value": op.pad_value}, {}),
+            lambda p, s, adir: ops.ListSlice(start=p["start"], end=p.get("end"), pad=p.get("pad", False),
+                                             pad_value=p.get("pad_value", 0.0))),
     }
 
 
