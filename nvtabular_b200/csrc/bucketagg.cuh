@@ -1,6 +1,6 @@
 // bucketagg.cuh — the group-by of a staged batch of a sorted accumulator WITHOUT a sort:
 // one order-free range partition + direct-address counting in shared memory.
-// Included by hashagg.cu after sortagg.cuh.
+// Included by sortacc.cu after partition.cuh.
 //
 // What it replaces: the LSD radix pipeline of sortagg.cuh (12-bit order-free pass + two STABLE
 // 10-bit passes + run-length encode) moved every key through HBM three times and spent most of
@@ -9,7 +9,7 @@
 //
 //   1. min / max of the valid keys (u = key ^ 2^31) -> lo, shift with (max - lo) >> shift < 2^13
 //   2. ONE order-free partition of v = u - lo by its top bits into 8192 buckets (the partition
-//      kernels of fold_i32.cuh: shared-memory counts, one global reservation per tile and bucket)
+//      kernels of partition.cuh: shared-memory counts, one global reservation per tile and bucket)
 //      — bucket b holds the keys of a window of 2^shift <= 2^19 consecutive values
 //   3. one CTA per bucket: a PRESENCE BITMAP of the window in shared memory (64 KB); a second
 //      bitmap marks the values seen twice; only those get a counter (dense index = popcount

@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -301,6 +302,11 @@ inline int scan_grid(int64_t n, int ctas_per_sm) {
   if (g > tiles) g = tiles;
   if (g < 1) g = 1;
   return (int)g;
+}
+
+// grid for a grid-stride loop of one item per thread: at most 8 CTAs per SM
+inline int plain_grid(int64_t n) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>((n + kThreads - 1) / kThreads, (int64_t)sm_count() * 8));
 }
 
 // ---------------------------------------------------------------------------

@@ -34,7 +34,7 @@
 #include <mutex>
 #include <new>
 
-#include "common.cuh"
+#include "hashagg.cuh"
 
 namespace nvtb {
 
@@ -82,13 +82,6 @@ struct Table {
   int narrow;
 };
 
-struct Counters {
-  unsigned long long n_unique;   // distinct keys in the table
-  unsigned long long size[2];    // special groups: [0] null key, [1] INT64_MIN key
-  unsigned long long ovf_count;  // pairs refused into the arena by the pending launch
-  unsigned long long max_count;  // sorted accumulator (sortagg.cuh): largest group size seen
-};
-
 struct Arena {
   int64_t* keys;
   int64_t* sizes;
@@ -115,23 +108,7 @@ struct nvtb_hashagg {
   int64_t hint;
   int n_agg;
   bool mailbox_valid;        // mailbox == device counters (no launch / host edit since the readback)
-  // sorted accumulator (sortagg.cuh), mode == 1: acc[acc_cur] holds ctr->n_unique packed pairs
-  int mode;                  // 0 = hash table, 1 = sorted runs
-  uint64_t* acc[2];
-  int64_t acc_cap[2];
-  int acc_cur;
-  uint32_t* d_n;             // device uint32[4]: [1] valid keys of the batch, [2] distinct keys of the batch
-  // staging of a sorted accumulator: batches are only COPIED (keys + validity bytes) until
-  // NVTB_STAGE_ROWS rows are waiting or somebody reads the handle; one sort + run-length
-  // encode + merge then takes all of them (a merge per batch re-reads and re-writes the
-  // whole accumulator, so its cost grows with every batch)
-  int32_t* stage_keys;
-  uint8_t* stage_mask;
-  int64_t stage_cap;         // rows
-  int64_t stage_rows;        // rows waiting (a multiple of 8 except after the last batch)
-  int64_t stage_hint;        // rows the previous fits staged: the buffer grows to hold one whole fit
-  cudaEvent_t stage_ev;
-  cudaStream_t stage_last;
+  nvtb::SortedAcc* acc;      // set once the handle has become a sorted accumulator (sortacc.cu); t is then unused
 };
 
 namespace nvtb {
@@ -314,12 +291,8 @@ __global__ void special_init_kernel(Counters* ctr, double* special_vals, int n_a
 }
 
 }  // namespace nvtb
+#include "partition.cuh"
 #include "fold_i32.cuh"
-namespace nvtb {
-constexpr int kExportPerThread = 4;
-}
-#include "sortagg.cuh"
-#include "bucketagg.cuh"
 namespace nvtb {
 
 // ---------------------------------------------------------------------------
@@ -716,6 +689,8 @@ rehash_kernel(Table old_t, Table new_t) {
   }
 }
 
+constexpr int kExportPerThread = 4;
+
 // compaction: table -> dense (unordered) arrays.  A CTA compacts 1024 slots at a time and
 // reserves its output range with ONE atomic: a per-warp atomicAdd on the single cursor
 // (500 k same-address atomics for a 16 M-slot table) serialised at ~1 ns each and cost
@@ -781,6 +756,53 @@ export_kernel(Table t, int64_t* __restrict__ keys_out,
     }
     __syncthreads();     // s_warp / s_base are reused by the next chunk
   }
+}
+
+// narrow hash table -> packed pairs (unordered); same per-CTA range reservation as export_kernel
+static __global__ void __launch_bounds__(kThreads)
+table_to_pairs_kernel(Table t, uint64_t* __restrict__ out, unsigned long long* cursor,
+                      unsigned long long* max_count) {
+  __shared__ unsigned s_warp[kThreads / 32];
+  __shared__ unsigned long long s_base;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  constexpr int64_t kChunk = (int64_t)kThreads * kExportPerThread;
+  uint32_t mx = 0;
+  for (int64_t c0 = (int64_t)blockIdx.x * kChunk; c0 < t.capacity; c0 += (int64_t)gridDim.x * kChunk) {
+    unsigned long long w[kExportPerThread];
+    unsigned live = 0;
+#pragma unroll
+    for (int j = 0; j < kExportPerThread; ++j) {
+      w[j] = (unsigned long long)t.slots[c0 + (int64_t)j * kThreads + threadIdx.x];
+      if (w[j] != 0ull) live |= 1u << j;
+    }
+    const unsigned mine = __popc(live);
+    unsigned incl = mine;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned y = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += y;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      unsigned tot = 0;
+      for (int q = 0; q < kThreads / 32; ++q) { const unsigned x = s_warp[q]; s_warp[q] = tot; tot += x; }
+      s_base = tot ? atomicAdd(cursor, (unsigned long long)tot) : 0ull;
+    }
+    __syncthreads();
+    int64_t o = (int64_t)s_base + s_warp[warp] + (incl - mine);
+#pragma unroll
+    for (int j = 0; j < kExportPerThread; ++j) {
+      if (!((live >> j) & 1u)) continue;
+      const uint32_t key = (uint32_t)w[j], cnt = (uint32_t)(w[j] >> 32);
+      out[o++] = ((uint64_t)(key ^ 0x80000000u) << 32) | cnt;
+      mx = cnt > mx ? cnt : mx;
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { const uint32_t y = __shfl_down_sync(0xFFFFFFFFu, mx, o); mx = y > mx ? y : mx; }
+  if (lane == 0 && mx) atomicMax(max_count, (unsigned long long)mx);
 }
 
 __global__ void decode_special_kernel(const double* special_vals, int n_agg,
@@ -909,10 +931,6 @@ pack_keys2_kernel(const int32_t* __restrict__ a, const uint8_t* __restrict__ ma,
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-static int plain_grid(int64_t n) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>((n + kThreads - 1) / kThreads, (int64_t)sm_count() * 8));
-}
-
 static int table_alloc(Table* t, int64_t capacity, int n_agg, bool narrow, cudaStream_t st) {
   t->capacity = capacity;
   t->n_agg = n_agg;
@@ -1139,8 +1157,34 @@ static int prepare(nvtb_hashagg* h, int64_t rows, cudaStream_t st) {
   return grow_to(h, want, st);
 }
 
-struct PartScratch { void* ptr; size_t bytes; cudaEvent_t ev; cudaStream_t last; bool used; };
-static PartScratch g_part = {nullptr, 0, nullptr, nullptr, false};
+int SharedScratch::acquire(size_t need, size_t alloc, cudaStream_t st, void** out, bool* grown) {
+  std::lock_guard<std::mutex> lk(mu);
+  *grown = false;
+  if (bytes < need) {
+    NVTB_CUDA_OK(cudaDeviceSynchronize());
+    if (ptr) cudaFree(ptr);
+    ptr = nullptr; bytes = 0;
+    NVTB_CUDA_OK(cudaMalloc(&ptr, alloc));
+    bytes = alloc;
+    used = false;               // the device is idle: no earlier use to wait for
+    *grown = true;
+  }
+  if (ev == nullptr) NVTB_CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  if (used && last != st) NVTB_CUDA_OK(cudaStreamWaitEvent(st, ev, 0));
+  *out = ptr;
+  return NVTB_OK;
+}
+
+int SharedScratch::release(cudaStream_t st) {
+  std::lock_guard<std::mutex> lk(mu);
+  NVTB_CUDA_OK(cudaEventRecord(ev, st));
+  used = true;
+  last = st;
+  return NVTB_OK;
+}
+
+// partition buffer of the PARTS mode
+static SharedScratch g_part;
 
 // int32 keys, narrow table, no payload: shared-memory fold, hash-partitioned first when the
 // expected number of distinct keys exceeds what one SM's shared memory holds (fold_i32.cuh)
@@ -1181,26 +1225,13 @@ static int launch_fold_i32(nvtb_hashagg* h, const int32_t* kp, const uint8_t* mp
   while ((1 << lg) < kMaxParts &&
          fresh / (double)(1 << lg) > kFoldMaxLoad * (double)(kFoldWays * kFoldBucketsParts)) ++lg;
   const int P = 1 << lg;
-  // partition buffer: ONE grow-only device allocation shared by every handle (a fresh
-  // 268 MB cudaMallocAsync per column occasionally costs tens of ms when the pool has to
-  // map new memory).  Uses are ordered by an event when the stream changes.
-  uint32_t* meta = nullptr;      // total[P] | starts[P] | cursor[P]
-  int32_t* buf = nullptr;
-  {
-    std::lock_guard<std::recursive_mutex> lk(g_arena_mu);
-    const size_t need = sizeof(uint32_t) * 3 * kMaxParts + sizeof(int32_t) * (size_t)(m + 8 * (int64_t)kMaxParts);
-    if (g_part.bytes < need) {
-      NVTB_CUDA_OK(cudaDeviceSynchronize());
-      if (g_part.ptr) cudaFree(g_part.ptr);
-      g_part.ptr = nullptr; g_part.bytes = 0;
-      NVTB_CUDA_OK(cudaMalloc(&g_part.ptr, need));
-      g_part.bytes = need;
-    }
-    if (g_part.ev == nullptr) NVTB_CUDA_OK(cudaEventCreateWithFlags(&g_part.ev, cudaEventDisableTiming));
-    if (g_part.used && g_part.last != st) NVTB_CUDA_OK(cudaStreamWaitEvent(st, g_part.ev, 0));
-    meta = reinterpret_cast<uint32_t*>(g_part.ptr);
-    buf = reinterpret_cast<int32_t*>(meta + 3 * kMaxParts);
-  }
+  const size_t need = sizeof(uint32_t) * 3 * kMaxParts + sizeof(int32_t) * (size_t)(m + 8 * (int64_t)kMaxParts);
+  void* part = nullptr;
+  bool grown = false;
+  int rc = g_part.acquire(need, need, st, &part, &grown);
+  if (rc) return rc;
+  uint32_t* meta = reinterpret_cast<uint32_t*>(part);      // total[P] | starts[P] | cursor[P]
+  int32_t* buf = reinterpret_cast<int32_t*>(meta + 3 * kMaxParts);
   NVTB_CUDA_OK(cudaMemsetAsync(meta, 0, sizeof(uint32_t) * P, st));
   const int64_t tiles = (m + kPartTile - 1) / kPartTile;
   part_hist_kernel<PartHashTop><<<(int)std::min<int64_t>(tiles, 3 * sms), kPartThreads, 4 * P, st>>>(
@@ -1215,18 +1246,12 @@ static int launch_fold_i32(nvtb_hashagg* h, const int32_t* kp, const uint8_t* mp
       buf, nullptr, m + 8 * (int64_t)P, meta + P, meta + 2 * P, P, 0, lg, kFoldBucketsParts, 1,
       h->t, h->ctr, h->arena);
   NVTB_LAUNCH_OK();
-  {
-    std::lock_guard<std::recursive_mutex> lk(g_arena_mu);
-    NVTB_CUDA_OK(cudaEventRecord(g_part.ev, st));
-    g_part.used = true;
-    g_part.last = st;
-  }
-  return NVTB_OK;
+  return g_part.release(st);
 }
 
 
 // ---------------------------------------------------------------------------------------
-// sorted accumulator (sortagg.cuh): host side
+// sorted accumulator (sortacc.cu)
 // ---------------------------------------------------------------------------------------
 // expected distinct keys above which an int32 column leaves the hash table for the sorted
 // accumulator: the table (2.5 slots x 8 B per key) then no longer stays in H100's 50 MB L2
@@ -1236,316 +1261,38 @@ static int64_t runs_min_keys() {
   return v < 1 ? 1 : v;
 }
 
-// ONE grow-only device scratch for the sort pipeline, shared by every handle of the process
-// (one process per GPU); uses on different streams are ordered by an event, like g_part
-struct SortScratch { void* ptr; size_t bytes; cudaEvent_t ev; cudaStream_t last; bool used; };
-static SortScratch g_sort = {nullptr, 0, nullptr, nullptr, false};
-
-struct SortCarve {
-  void* rx;                  // radix scratch; its first 256 B are kept at zero
-  size_t rx_bytes;
-  uint32_t* part_meta;       // total[P] | starts[P] | cursor[P]
-  uint32_t* keys_a;
-  uint32_t* keys_b;
-  uint64_t* rle;             // [m + 1]
-  uint32_t* tile_heads;      // [ceil(m / kRleTile)]
-  uint2* splits;             // [MT + 1]
-  uint32_t* tile_out;        // [MT]
-};
-
-static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-static int sort_scratch_acquire(int64_t m, int64_t n_pairs_sort, int64_t mt, cudaStream_t st, SortCarve* c) {
-  const int P = 1 << kSortLowBits;
-  const size_t rx_bytes = align_up(std::max(rx_scratch_bytes<uint32_t>(m), rx_scratch_bytes<uint64_t>(n_pairs_sort)), 256);
-  // radix path: total[P] | starts[P] | cursor[P]; bucket path (bucketagg.cuh): the same three with
-  // 8192 entries + distinct[8192] + {min, max, lo, shift, flag}
-  const size_t meta_bytes = align_up(sizeof(uint32_t) * (size_t)std::max(3 * P, 4 * kBkParts + 64), 256);
-  const size_t keys_bytes = align_up(sizeof(uint32_t) * (size_t)(m + 64), 256);
-  const size_t rle_bytes = align_up(sizeof(uint64_t) * (size_t)(m + 2), 256);
-  const size_t heads_bytes = align_up(sizeof(uint32_t) * (size_t)((m + kRleTile - 1) / kRleTile + 1), 256);
-  const size_t splits_bytes = align_up(sizeof(uint2) * (size_t)(mt + 2), 256);
-  const size_t out_bytes = align_up(sizeof(uint32_t) * (size_t)(mt + 2), 256);
-  const size_t need = rx_bytes + meta_bytes + 2 * keys_bytes + rle_bytes + heads_bytes + splits_bytes + out_bytes;
-  std::lock_guard<std::recursive_mutex> lk(g_arena_mu);
-  if (g_sort.bytes < need) {
-    NVTB_CUDA_OK(cudaDeviceSynchronize());
-    if (g_sort.ptr) cudaFree(g_sort.ptr);
-    g_sort.ptr = nullptr; g_sort.bytes = 0;
-    const size_t want = need + need / 8;
-    NVTB_CUDA_OK(cudaMalloc(&g_sort.ptr, want));
-    g_sort.bytes = want;
-    NVTB_CUDA_OK(cudaMemsetAsync(g_sort.ptr, 0, 256, st));
-    g_sort.used = false;
-  }
-  if (g_sort.ev == nullptr) NVTB_CUDA_OK(cudaEventCreateWithFlags(&g_sort.ev, cudaEventDisableTiming));
-  if (g_sort.used && g_sort.last != st) NVTB_CUDA_OK(cudaStreamWaitEvent(st, g_sort.ev, 0));
-  char* p = reinterpret_cast<char*>(g_sort.ptr);
-  c->rx = p;                                         p += rx_bytes;
-  c->rx_bytes = rx_bytes;
-  c->part_meta = reinterpret_cast<uint32_t*>(p);     p += meta_bytes;
-  c->keys_a = reinterpret_cast<uint32_t*>(p);        p += keys_bytes;
-  c->keys_b = reinterpret_cast<uint32_t*>(p);        p += keys_bytes;
-  c->rle = reinterpret_cast<uint64_t*>(p);           p += rle_bytes;
-  c->tile_heads = reinterpret_cast<uint32_t*>(p);    p += heads_bytes;
-  c->splits = reinterpret_cast<uint2*>(p);           p += splits_bytes;
-  c->tile_out = reinterpret_cast<uint32_t*>(p);
-  return NVTB_OK;
-}
-
-static int sort_scratch_release(cudaStream_t st) {
-  std::lock_guard<std::recursive_mutex> lk(g_arena_mu);
-  NVTB_CUDA_OK(cudaEventRecord(g_sort.ev, st));
-  g_sort.used = true;
-  g_sort.last = st;
-  return NVTB_OK;
-}
-
-// make sure acc[which] can hold `pairs` packed pairs (contents are NOT preserved)
-static int acc_reserve(nvtb_hashagg* h, int which, int64_t pairs, cudaStream_t st) {
-  if (h->acc_cap[which] >= pairs) return NVTB_OK;
-  if (h->acc[which]) NVTB_CUDA_OK(cudaFreeAsync(h->acc[which], st));
-  h->acc[which] = nullptr; h->acc_cap[which] = 0;
-  const int64_t want = pairs + pairs / 8 + 1024;
-  NVTB_CUDA_OK(cudaMallocAsync(&h->acc[which], sizeof(uint64_t) * (size_t)want, st));
-  h->acc_cap[which] = want;
-  return NVTB_OK;
-}
-
-// hash table -> sorted accumulator (the handle must be settled and its table narrow).
-// One-off: export the u_known (key, count) pairs packed and sort them by key.
+// hash table -> sorted accumulator (the handle must be settled and its table narrow): the
+// u_known (key, count) pairs are exported into the accumulator, which sorts them by key
 static int table_to_runs(nvtb_hashagg* h, cudaStream_t st) {
   const int64_t nu = h->u_known;
-  if (h->d_n == nullptr) {
-    NVTB_CUDA_OK(cudaMalloc(&h->d_n, sizeof(uint32_t) * 4));
-    NVTB_CUDA_OK(cudaMemsetAsync(h->d_n, 0, sizeof(uint32_t) * 4, st));
-  }
-  h->acc_cur = 0;
+  uint64_t* pairs = nullptr;
+  int rc = sortacc_create(&h->acc, nu, st, &pairs);
+  if (rc) return rc;
   if (nu > 0) {
-    int rc = acc_reserve(h, 0, nu, st);
-    if (rc) return rc;
-    rc = acc_reserve(h, 1, nu, st);
-    if (rc) return rc;
-    SortCarve c;
-    rc = sort_scratch_acquire(64, nu, 1, st, &c);
-    if (rc) return rc;
-    unsigned long long* cursor = reinterpret_cast<unsigned long long*>(c.part_meta);
+    unsigned long long* cursor = nullptr;
+    NVTB_CUDA_OK(cudaMallocAsync(&cursor, sizeof(unsigned long long), st));
     NVTB_CUDA_OK(cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), st));
     table_to_pairs_kernel<<<plain_grid(h->t.capacity / kExportPerThread), kThreads, 0, st>>>(
-        h->t, h->acc[0], cursor, &h->ctr->max_count);
+        h->t, pairs, cursor, &h->ctr->max_count);
     NVTB_LAUNCH_OK();
-    int in_b = 0;
-    rc = rx_sort_bits<uint64_t>(nullptr, h->acc[0], h->acc[1], nullptr, nu, 32, 64, false, c.rx, c.rx_bytes, st, &in_b);
-    if (rc) return rc;
-    h->acc_cur = in_b;
-    rc = sort_scratch_release(st);
+    NVTB_CUDA_OK(cudaFreeAsync(cursor, st));
+    rc = sortacc_sort_pairs(h->acc, nu, st);
     if (rc) return rc;
   }
   // the table itself is no longer used: keep a minimal one so that the handle stays uniform
-  int rc = table_free(&h->t, st);
+  rc = table_free(&h->t, st);
   if (rc) return rc;
-  rc = table_alloc(&h->t, kMinCapacity, 0, true, st);
-  if (rc) return rc;
-  h->mode = 1;
-  return NVTB_OK;
+  return table_alloc(&h->t, kMinCapacity, 0, true, st);
 }
 
-// fold one batch of int32 keys into the sorted accumulator (handle settled: u_known exact)
-static int launch_runs_insert(nvtb_hashagg* h, const int32_t* kp, const uint8_t* mp, int64_t m, cudaStream_t st) {
-  static bool attrs = false;
-  constexpr int kScatterSmem = kPartTile * 4 + 2 * 4 * (1 << kSortLowBits);
-  if (!attrs) {
-    NVTB_CUDA_OK(cudaFuncSetAttribute(part_scatter_kernel<PartKeyLow>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, kScatterSmem));
-    NVTB_CUDA_OK(cudaFuncSetAttribute(merge_write_kernel<false>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MergeSmem)));
-    NVTB_CUDA_OK(cudaFuncSetAttribute(merge_write_kernel<true>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MergeSmem)));
-    attrs = true;
-  }
-  const int64_t ua = h->u_known;
-  const int other = h->acc_cur ^ 1;
-  int rc = NVTB_OK;
-  const int64_t mt = (ua + m + kMergeTile - 1) / kMergeTile;
-  SortCarve c;
-  rc = sort_scratch_acquire(m, 64, mt, st, &c);
-  if (rc) return rc;
-  const int sms = sm_count();
-  const int P = 1 << kSortLowBits;
-  const int aligned = is_aligned32(kp) ? 1 : 0;
-  uint32_t* n_valid = h->d_n + 1;
-  uint32_t* n_batch = h->d_n + 2;
-  const int64_t tiles = (m + kPartTile - 1) / kPartTile;
-  const uint64_t* A = h->acc[h->acc_cur];
-  // ---- bucket path (bucketagg.cuh): range partition + direct-address counting, no sort ----------
-  bool done = false;
-  const char* path_env = getenv("NVTB_SORT_PATH");
-  if (!(path_env && strcmp(path_env, "radix") == 0)) {
-    static bool bk_attrs = false;
-    constexpr int kBkScatterSmem = kPartTile * 4 + 2 * 4 * kBkParts;
-    if (!bk_attrs) {
-      NVTB_CUDA_OK(cudaFuncSetAttribute(part_hist_kernel<PartRange>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kBkParts));
-      NVTB_CUDA_OK(cudaFuncSetAttribute(part_scatter_kernel<PartRange>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBkScatterSmem));
-      NVTB_CUDA_OK(cudaFuncSetAttribute(bk_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kBkCountSmem));
-      NVTB_CUDA_OK(cudaFuncSetAttribute(bk_emit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kBkEmitSmem));
-      bk_attrs = true;
-    }
-    uint32_t* total = c.part_meta;                    // -> exclusive starts after the scan
-    uint32_t* cursor = c.part_meta + kBkParts;
-    uint32_t* distinct = c.part_meta + 2 * kBkParts;  // -> output offsets after the scan
-    uint32_t* mm = c.part_meta + 4 * kBkParts;        // {min, max}
-    uint32_t* par = mm + 2;                           // {lo, shift}
-    unsigned int* flag = reinterpret_cast<unsigned int*>(mm + 4);
-    const uint32_t mm_init[6] = {0xFFFFFFFFu, 0u, 0u, 0u, 0u, 0u};
-    NVTB_CUDA_OK(cudaMemcpyAsync(mm, mm_init, sizeof(mm_init), cudaMemcpyHostToDevice, st));
-    NVTB_CUDA_OK(cudaMemsetAsync(total, 0, sizeof(uint32_t) * kBkParts, st));
-    bk_minmax_kernel<<<(int)std::min<int64_t>(tiles, 4 * sms), kPartThreads, 0, st>>>(kp, mp, m, mm, aligned);
-    NVTB_LAUNCH_OK();
-    bk_params_kernel<<<1, 1, 0, st>>>(mm, par);
-    NVTB_LAUNCH_OK();
-    const PartRange pol{kBkLgParts, par};
-    part_hist_kernel<PartRange><<<(int)std::min<int64_t>(tiles, 3 * sms), kPartThreads, 4 * kBkParts, st>>>(
-        kp, mp, m, pol, total, h->ctr, aligned);
-    NVTB_LAUNCH_OK();
-    scan_tiles_kernel<<<1, kRunThreads, 0, st>>>(total, kBkParts, n_valid, nullptr);
-    NVTB_LAUNCH_OK();
-    NVTB_CUDA_OK(cudaMemcpyAsync(cursor, total, sizeof(uint32_t) * kBkParts, cudaMemcpyDeviceToDevice, st));
-    part_scatter_kernel<PartRange><<<(int)std::min<int64_t>(tiles, sms), kPartThreads, kBkScatterSmem, st>>>(
-        kp, mp, m, pol, cursor, reinterpret_cast<int32_t*>(c.keys_a), aligned);
-    NVTB_LAUNCH_OK();
-    bk_count_kernel<<<kBkParts, kBkThreads, kBkCountSmem, st>>>(c.keys_a, total, n_valid, par, distinct);
-    NVTB_LAUNCH_OK();
-    scan_tiles_kernel<<<1, kRunThreads, 0, st>>>(distinct, kBkParts, n_batch, ua == 0 ? &h->ctr->n_unique : nullptr);
-    NVTB_LAUNCH_OK();
-    // the accumulator is sized for what the batch really holds (its distinct keys are known now),
-    // not for the worst case of all rows distinct
-    uint32_t nb_h = 0;
-    NVTB_CUDA_OK(cudaMemcpyAsync(&nb_h, n_batch, sizeof(nb_h), cudaMemcpyDeviceToHost, st));
-    NVTB_CUDA_OK(cudaStreamSynchronize(st));
-    rc = acc_reserve(h, other, ua + (int64_t)nb_h, st);
-    if (rc) return rc;
-    // the batch's pairs go straight into the accumulator when it is empty, else to the merge input
-    uint64_t* B = (ua == 0) ? h->acc[other] : c.rle;
-    bk_emit_kernel<<<kBkParts, kBkThreads, kBkEmitSmem, st>>>(c.keys_a, total, n_valid, par, distinct, B, flag,
-                                                               &h->ctr->max_count);
-    NVTB_LAUNCH_OK();
-    unsigned int flag_h = 0;
-    NVTB_CUDA_OK(cudaMemcpyAsync(&flag_h, flag, sizeof(flag_h), cudaMemcpyDeviceToHost, st));
-    NVTB_CUDA_OK(cudaStreamSynchronize(st));
-    if (flag_h == 0) {
-      if (ua > 0) {
-        merge_split_kernel<<<(int)((mt + 1 + 255) / 256), 256, 0, st>>>(A, (uint32_t)ua, B, n_batch, (int)mt, c.splits);
-        NVTB_LAUNCH_OK();
-        merge_count_kernel<<<(int)mt, kRunThreads, 0, st>>>(A, B, c.splits, c.tile_out);
-        NVTB_LAUNCH_OK();
-        scan_tiles_kernel<<<1, kRunThreads, 0, st>>>(c.tile_out, (int)mt, nullptr, &h->ctr->n_unique);
-        NVTB_LAUNCH_OK();
-        merge_write_kernel<true><<<(int)mt, kRunThreads, sizeof(MergeSmem), st>>>(A, B, c.splits, c.tile_out, h->acc[other],
-                                                                                  &h->ctr->max_count);
-        NVTB_LAUNCH_OK();
-      }
-      done = true;
-    }
-    // flag set: some window holds more than kBkDupCap duplicated values -> the radix pipeline
-    // below redoes the batch (the nulls have been counted already)
-  }
-  if (!done) {
-    rc = acc_reserve(h, other, ua + m, st);
-    if (rc) return rc;
-    Counters* null_ctr = (path_env && strcmp(path_env, "radix") == 0) ? h->ctr : nullptr;
-    // (1) LSD radix sort of the valid keys (as key ^ 2^31)
-    NVTB_CUDA_OK(cudaMemsetAsync(c.part_meta, 0, sizeof(uint32_t) * P, st));
-    part_hist_kernel<PartKeyLow><<<(int)std::min<int64_t>(tiles, 3 * sms), kPartThreads, 4 * P, st>>>(
-        kp, mp, m, PartKeyLow{kSortLowBits}, c.part_meta, null_ctr, aligned);
-    NVTB_LAUNCH_OK();
-    part_scan_kernel<<<1, kPartThreads, 0, st>>>(c.part_meta, kSortLowBits, c.part_meta + P, c.part_meta + 2 * P, 1u, n_valid);
-    NVTB_LAUNCH_OK();
-    part_scatter_kernel<PartKeyLow><<<(int)std::min<int64_t>(tiles, 2 * sms), kPartThreads, kScatterSmem, st>>>(
-        kp, mp, m, PartKeyLow{kSortLowBits}, c.part_meta + 2 * P, reinterpret_cast<int32_t*>(c.keys_a), aligned);
-    NVTB_LAUNCH_OK();
-    int in_b = 0;
-    rc = rx_sort_bits<uint32_t>(nullptr, c.keys_a, c.keys_b, n_valid, m, kSortLowBits, 32, false, c.rx, c.rx_bytes, st,
-                               &in_b);
-    if (rc) return rc;
-    const uint32_t* sorted = in_b ? c.keys_b : c.keys_a;
-    // (2) run heads
-    const int rt = (int)((m + kRleTile - 1) / kRleTile);
-    rle_count_kernel<<<rt, kRunThreads, 0, st>>>(sorted, n_valid, m, c.tile_heads);
-    NVTB_LAUNCH_OK();
-    scan_tiles_kernel<<<1, kRunThreads, 0, st>>>(c.tile_heads, rt, n_batch, nullptr);
-    NVTB_LAUNCH_OK();
-    rle_write_kernel<<<rt, kRunThreads, 0, st>>>(sorted, n_valid, m, c.tile_heads, n_batch, c.rle);
-    NVTB_LAUNCH_OK();
-    // (3) merge with the accumulator
-    merge_split_kernel<<<(int)((mt + 1 + 255) / 256), 256, 0, st>>>(A, (uint32_t)ua, c.rle, n_batch, (int)mt, c.splits);
-    NVTB_LAUNCH_OK();
-    merge_count_kernel<<<(int)mt, kRunThreads, 0, st>>>(A, c.rle, c.splits, c.tile_out);
-    NVTB_LAUNCH_OK();
-    scan_tiles_kernel<<<1, kRunThreads, 0, st>>>(c.tile_out, (int)mt, nullptr, &h->ctr->n_unique);
-    NVTB_LAUNCH_OK();
-    merge_write_kernel<false><<<(int)mt, kRunThreads, sizeof(MergeSmem), st>>>(A, c.rle, c.splits, c.tile_out, h->acc[other],
-                                                                               &h->ctr->max_count);
-    NVTB_LAUNCH_OK();
-  }
-  h->acc_cur = other;
-  return sort_scratch_release(st);
-}
-
-// rows a sorted accumulator stages before it sorts (NVTB_STAGE_ROWS, default 2^28 = 1 GiB of keys)
-static int64_t stage_cap_rows() {
-  const char* e = getenv("NVTB_STAGE_ROWS");
-  int64_t v = e ? atoll(e) : ((int64_t)1 << 28);
-  if (v < 0) v = 0;
-  if (v > (int64_t)0xF0000000ll) v = (int64_t)0xF0000000ll;
-  return v / 64 * 64;
-}
-
-// sort + run-length encode + merge everything that is staged (handle settled on entry; leaves a
-// pending launch)
-static int post(nvtb_hashagg* h, cudaStream_t st);
-static int stage_flush(nvtb_hashagg* h, cudaStream_t st) {
-  if (h->stage_rows == 0) return NVTB_OK;
+// group + merge the batches a sorted accumulator has staged (leaves a pending launch)
+static int acc_flush(nvtb_hashagg* h, cudaStream_t st) {
+  if (h->acc == nullptr || sortacc_staged_rows(h->acc) == 0) return NVTB_OK;
   int rc = settle(h);
   if (rc) return rc;
-  if (h->stage_last != st && h->stage_ev) NVTB_CUDA_OK(cudaStreamWaitEvent(st, h->stage_ev, 0));
-  rc = launch_runs_insert(h, h->stage_keys, h->stage_mask, h->stage_rows, st);
+  rc = sortacc_flush(h->acc, h->u_known, h->ctr, st);
   if (rc) return rc;
-  h->stage_rows = 0;
-  NVTB_CUDA_OK(cudaEventRecord(h->stage_ev, st));
-  h->stage_last = st;
   return post(h, st);
-}
-
-// append one batch to the staging buffers (stage_rows % 8 == 0; the caller flushed when the
-// batch does not fit behind the waiting rows)
-static int stage_append(nvtb_hashagg* h, const int32_t* kp, const uint8_t* mp, int64_t m, cudaStream_t st) {
-  if (h->stage_ev == nullptr) NVTB_CUDA_OK(cudaEventCreateWithFlags(&h->stage_ev, cudaEventDisableTiming));
-  if (h->stage_last != nullptr && h->stage_last != st) NVTB_CUDA_OK(cudaStreamWaitEvent(st, h->stage_ev, 0));
-  const int64_t cap_max = stage_cap_rows();
-  const bool grow_for_fit = h->stage_rows == 0 && h->stage_cap < std::min<int64_t>(cap_max, h->stage_hint);
-  if (h->stage_rows + m > h->stage_cap || grow_for_fit) {
-    NVTB_REQUIRE(h->stage_rows == 0, "staging buffer resized while rows are waiting");
-    if (h->stage_keys) NVTB_CUDA_OK(cudaFreeAsync(h->stage_keys, st));
-    if (h->stage_mask) NVTB_CUDA_OK(cudaFreeAsync(h->stage_mask, st));
-    h->stage_keys = nullptr; h->stage_mask = nullptr; h->stage_cap = 0;
-    // sized for what the fit has shown so far (a small fit must not pay for 1 GiB), doubling
-    const int64_t cap = cap_max;
-    int64_t want = std::max<int64_t>((int64_t)1 << 22, next_pow2(2 * (h->rows_total + m)));
-    want = std::max<int64_t>(want, (h->stage_hint + 63) / 64 * 64);      // one flush per fit from the second fit on
-    want = std::max<int64_t>(std::min<int64_t>(want, cap), m);
-    NVTB_CUDA_OK(cudaMallocAsync(&h->stage_keys, sizeof(int32_t) * (size_t)(want + 64), st));
-    NVTB_CUDA_OK(cudaMallocAsync(&h->stage_mask, (size_t)(want / 8 + 64), st));
-    h->stage_cap = want;
-  }
-  NVTB_CUDA_OK(cudaMemcpyAsync(h->stage_keys + h->stage_rows, kp, sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToDevice, st));
-  uint8_t* md = h->stage_mask + (h->stage_rows >> 3);
-  const size_t mbytes = (size_t)((m + 7) >> 3);
-  if (mp) NVTB_CUDA_OK(cudaMemcpyAsync(md, mp, mbytes, cudaMemcpyDeviceToDevice, st));
-  else    NVTB_CUDA_OK(cudaMemsetAsync(md, 0xFF, mbytes, st));
-  h->stage_rows += m;
-  NVTB_CUDA_OK(cudaEventRecord(h->stage_ev, st));
-  h->stage_last = st;
-  return NVTB_OK;
 }
 
 template <typename KeyT>
@@ -1580,8 +1327,6 @@ static int launch_insert(nvtb_hashagg* h, const KeyT* kp, const uint8_t* mp, con
   return post(h, st);
 }
 
-// view of a handle for nvtb_vocab_build_from_hashagg (vocab.cu): synchronises on the handle's
-// pending launch.  *pairs == nullptr when the handle is a hash table (the caller exports).
 int hashagg_sorted_view(nvtb_hashagg* h, const uint64_t** pairs, int64_t* n_unique, int64_t* null_size,
                         uint64_t* max_count, int* is_i32_table, cudaStream_t st) {
   int64_t nu = 0, ns = 0;
@@ -1590,8 +1335,8 @@ int hashagg_sorted_view(nvtb_hashagg* h, const uint64_t** pairs, int64_t* n_uniq
   *n_unique = nu;
   *null_size = ns;
   *max_count = (uint64_t)h->mailbox->max_count;
-  *pairs = h->mode == 1 ? h->acc[h->acc_cur] : nullptr;
-  *is_i32_table = (h->mode == 0 && h->t.narrow) ? 1 : 0;
+  *pairs = h->acc ? sortacc_pairs(h->acc) : nullptr;
+  *is_i32_table = (!h->acc && h->t.narrow) ? 1 : 0;
   return NVTB_OK;
 }
 
@@ -1632,16 +1377,15 @@ int nvtb_hashagg_reset(nvtb_hashagg_t* h, void* stream) {
   // the table keeps its capacity (and the estimate its value): a second fit over
   // similar data needs no growth and no sampling pass
   h->hint = std::max<int64_t>(h->hint, h->u_known);
-  if (h->mode == 0) {      // a sorted accumulator is emptied by zeroing its counters below
+  if (h->acc == nullptr) {      // a sorted accumulator is emptied by zeroing its counters below
     table_init_kernel<<<plain_grid(h->t.capacity), kThreads, 0, st>>>(h->t);
     NVTB_LAUNCH_OK();
   }
   special_init_kernel<<<1, 32, 0, st>>>(h->ctr, h->special_vals, h->n_agg);
   NVTB_LAUNCH_OK();
-  h->stage_hint = std::max<int64_t>(h->stage_hint, h->rows_total);   // the fit that just ended
+  if (h->acc) sortacc_reset(h->acc, h->rows_total);
   h->u_known = 0;
   h->rows_total = 0;
-  h->stage_rows = 0;          // batches still waiting belong to the fit that is being discarded
   h->mailbox_valid = false;
   return NVTB_OK;
 }
@@ -1656,12 +1400,7 @@ int nvtb_hashagg_destroy(nvtb_hashagg_t* h) {
   if (h->special_vals) cudaFree(h->special_vals);
   if (h->mailbox) cudaFreeHost(h->mailbox);
   if (h->ev) cudaEventDestroy(h->ev);
-  if (h->acc[0]) cudaFree(h->acc[0]);
-  if (h->acc[1]) cudaFree(h->acc[1]);
-  if (h->d_n) cudaFree(h->d_n);
-  if (h->stage_keys) cudaFree(h->stage_keys);
-  if (h->stage_mask) cudaFree(h->stage_mask);
-  if (h->stage_ev) cudaEventDestroy(h->stage_ev);
+  if (h->acc) sortacc_destroy(h->acc);
   delete h;
   return NVTB_OK;
 }
@@ -1689,7 +1428,7 @@ int nvtb_hashagg_insert(nvtb_hashagg_t* h, const nvtb_col_t* key,
     if (rc) return rc;
     const bool can_narrow = h->n_agg == 0 && key->dtype == NVTB_I32 &&
                             h->rows_total + n < (int64_t)0xFFFFFFF0ll;
-    if (h->mode == 1) {
+    if (h->acc) {
       // sorted accumulator: nothing to switch
     } else if (h->rows_total == 0 && h->u_known == 0 && can_narrow && !h->t.narrow) {
       // empty table: switch to the 8-byte layout in place
@@ -1709,12 +1448,12 @@ int nvtb_hashagg_insert(nvtb_hashagg_t* h, const nvtb_col_t* key,
     int rc = settle(h);
     if (rc) return rc;
     int64_t m = n - off;
-    const bool blind = (h->mode == 0 && h->hint == 0 && h->k_est == 0);
+    const bool blind = (h->acc == nullptr && h->hint == 0 && h->k_est == 0);
     if (blind && m > 4 * kSampleRows) m = kSampleRows;
     const void* kp = (const char*)key->data + off * ksz;
     const uint8_t* mp = key->validity ? key->validity + (off >> 3) : nullptr;  // off % 8 == 0
-    if (h->mode == 0) {
-      // a column whose table would leave the L2 moves to the sorted accumulator (sortagg.cuh)
+    if (h->acc == nullptr) {
+      // a column whose table would leave the L2 moves to the sorted accumulator (sortacc.cu)
       predict(h, m);
       const bool eligible = h->n_agg == 0 && key->dtype == NVTB_I32 && h->t.narrow &&
                             h->rows_total + n < (int64_t)0xFFFFFFF0ll && m < (int64_t)0xFFFF0000ll;
@@ -1723,32 +1462,27 @@ int nvtb_hashagg_insert(nvtb_hashagg_t* h, const nvtb_col_t* key,
         if (rc) return rc;
       }
     }
-    if (h->mode == 1) {
+    if (h->acc) {
       NVTB_REQUIRE(h->n_agg == 0 && key->dtype == NVTB_I32, "a sorted accumulator takes int32 keys without payload");
       NVTB_REQUIRE(h->rows_total + m < (int64_t)0xFFFFFFF0ll, "more than 2^32 rows in one int32 accumulator");
-      int64_t mm = m < (int64_t)0xFFFF0000ll ? m : (int64_t)0x80000000ll;
-      const int64_t cap = stage_cap_rows();
-      if (cap >= 64 && mm <= cap && (h->stage_rows & 7) == 0) {
-        // stage: copy now, sort later together with the other batches of this fit
-        if (h->stage_rows + mm > h->stage_cap && h->stage_rows > 0) {
-          rc = stage_flush(h, st);
-          if (rc) return rc;
-        }
-        rc = stage_append(h, (const int32_t*)kp, mp, mm, st);
+      const int64_t mm = m < (int64_t)0xFFFF0000ll ? m : (int64_t)0x80000000ll;
+      const bool stage = sortacc_stages(h->acc, mm);
+      if (!stage || sortacc_stage_full(h->acc, mm)) {
+        rc = acc_flush(h, st);
         if (rc) return rc;
-        h->rows_total += mm;
-        off += mm;
-        continue;
       }
-      rc = stage_flush(h, st);            // ragged tail waiting, or a batch larger than the stage
-      if (rc) return rc;
-      rc = settle(h);
-      if (rc) return rc;
-      rc = launch_runs_insert(h, (const int32_t*)kp, mp, mm, st);
-      if (rc) return rc;
+      if (stage) {                        // copy now, sort later together with the other batches of this fit
+        rc = sortacc_stage(h->acc, (const int32_t*)kp, mp, mm, h->rows_total, st);
+        if (rc) return rc;
+      } else {                            // ragged tail waiting, or a batch larger than the stage
+        rc = settle(h);
+        if (rc) return rc;
+        rc = sortacc_insert(h->acc, (const int32_t*)kp, mp, mm, h->u_known, h->ctr, st);
+        if (rc) return rc;
+        rc = post(h, st);
+        if (rc) return rc;
+      }
       h->rows_total += mm;
-      rc = post(h, st);
-      if (rc) return rc;
       off += mm;
       continue;
     }
@@ -1777,7 +1511,7 @@ int nvtb_hashagg_merge(nvtb_hashagg_t* h, const int64_t* keys,
   cudaStream_t st = (cudaStream_t)stream;
   int rc = settle(h);
   if (rc) return rc;
-  if (h->mode == 1) {
+  if (h->acc) {
     set_error("nvtb_hashagg_merge: the handle holds a sorted accumulator (raw int32 rows only)");
     return NVTB_ESTATE;
   }
@@ -1829,8 +1563,8 @@ int nvtb_hashagg_size(nvtb_hashagg_t* h, int64_t* n_unique, int64_t* null_size, 
   cudaStream_t st = (cudaStream_t)stream;
   int rc = settle(h);
   if (rc) return rc;
-  if (h->stage_rows > 0) {   // a sorted accumulator with batches still waiting: sort them in now
-    rc = stage_flush(h, st);
+  if (h->acc && sortacc_staged_rows(h->acc) > 0) {   // batches still waiting: group them in now
+    rc = acc_flush(h, st);
     if (rc) return rc;
     rc = settle(h);
     if (rc) return rc;
@@ -1869,11 +1603,7 @@ int nvtb_hashagg_export(nvtb_hashagg_t* h, int64_t* keys_out, int64_t* sizes_out
   if (nu == 0) return NVTB_OK;
   NVTB_REQUIRE(keys_out != nullptr, "keys_out is NULL");
   NVTB_REQUIRE(h->n_agg == 0 || vals_out != nullptr, "vals_out is NULL");
-  if (h->mode == 1) {      // sorted accumulator: unpack (the rows come out in key order)
-    runs_unpack_kernel<<<plain_grid(nu), kThreads, 0, st>>>(h->acc[h->acc_cur], nu, keys_out, sizes_out);
-    NVTB_LAUNCH_OK();
-    return NVTB_OK;
-  }
+  if (h->acc) return sortacc_unpack(h->acc, nu, keys_out, sizes_out, st);   // the rows come out in key order
   unsigned long long* cursor = nullptr;
   NVTB_CUDA_OK(cudaMallocAsync(&cursor, sizeof(unsigned long long), st));
   NVTB_CUDA_OK(cudaMemsetAsync(cursor, 0, sizeof(unsigned long long), st));
@@ -1893,46 +1623,8 @@ int nvtb_hashagg_export(nvtb_hashagg_t* h, int64_t* keys_out, int64_t* sizes_out
   return NVTB_OK;
 }
 
-// Stable LSD radix sort of bits [lo_bit, hi_bit) (radix.cuh), exposed for tests and for
-// callers that order their own device arrays.  The result ends in `data` or in `tmp`
-// (*result_in_tmp_host).
-static int radix_sort_entry(void* data, void* tmp, int64_t n, int elem_bytes, int lo_bit, int hi_bit,
-                            int descending, int* result_in_tmp_host, void* stream) {
-  NVTB_REQUIRE(n >= 0 && result_in_tmp_host != nullptr, "bad n / NULL result flag");
-  NVTB_REQUIRE(lo_bit >= 0 && hi_bit <= 8 * elem_bytes && lo_bit <= hi_bit, "bad bit range");
-  *result_in_tmp_host = 0;
-  if (n == 0 || lo_bit == hi_bit) return NVTB_OK;
-  NVTB_REQUIRE(data != nullptr && tmp != nullptr, "NULL data/tmp");
-  NVTB_REQUIRE((reinterpret_cast<uintptr_t>(data) & 15u) == 0 && (reinterpret_cast<uintptr_t>(tmp) & 15u) == 0,
-               "data/tmp must be 16-byte aligned");
-  cudaStream_t st = (cudaStream_t)stream;
-  void* scratch = nullptr;
-  const size_t bytes = elem_bytes == 4 ? rx_scratch_bytes<uint32_t>(n) : rx_scratch_bytes<uint64_t>(n);
-  NVTB_CUDA_OK(cudaMallocAsync(&scratch, bytes, st));
-  NVTB_CUDA_OK(cudaMemsetAsync(scratch, 0, 256, st));
-  int rc;
-  if (elem_bytes == 4)
-    rc = rx_sort_bits<uint32_t>(nullptr, (uint32_t*)data, (uint32_t*)tmp, nullptr, n, lo_bit, hi_bit, descending != 0,
-                                scratch, bytes, st, result_in_tmp_host);
-  else
-    rc = rx_sort_bits<uint64_t>(nullptr, (uint64_t*)data, (uint64_t*)tmp, nullptr, n, lo_bit, hi_bit, descending != 0,
-                                scratch, bytes, st, result_in_tmp_host);
-  NVTB_CUDA_OK(cudaFreeAsync(scratch, st));
-  return rc;
-}
-
-int nvtb_radix_sort_u32(uint32_t* data, uint32_t* tmp, int64_t n, int lo_bit, int hi_bit, int descending,
-                        int* result_in_tmp_host, void* stream) {
-  return radix_sort_entry(data, tmp, n, 4, lo_bit, hi_bit, descending, result_in_tmp_host, stream);
-}
-
-int nvtb_radix_sort_u64(uint64_t* data, uint64_t* tmp, int64_t n, int lo_bit, int hi_bit, int descending,
-                        int* result_in_tmp_host, void* stream) {
-  return radix_sort_entry(data, tmp, n, 8, lo_bit, hi_bit, descending, result_in_tmp_host, stream);
-}
-
 // ---------------------------------------------------------------------------------------
-// sorted-pair primitives of the cross-GPU vocabulary merge (nvtabular_b200/dist.py)
+// sorted accumulators in the cross-GPU vocabulary merge (nvtabular_b200/dist.py)
 // ---------------------------------------------------------------------------------------
 // Turn an int32 key-count handle into a sorted accumulator (no-op when it already is one), so
 // that every rank of a fit holds the same representation of a high-cardinality column.
@@ -1941,7 +1633,7 @@ int nvtb_hashagg_to_sorted(nvtb_hashagg_t* h, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   int rc = settle(h);
   if (rc) return rc;
-  if (h->mode == 1) return NVTB_OK;
+  if (h->acc) return NVTB_OK;
   int64_t nu = 0, ns = 0;
   rc = nvtb_hashagg_size(h, &nu, &ns, stream);
   if (rc) return rc;
@@ -1961,89 +1653,14 @@ int nvtb_hashagg_export_packed(nvtb_hashagg_t* h, uint64_t* out, int64_t* n_host
   int64_t nu = 0, ns = 0;
   int rc = nvtb_hashagg_size(h, &nu, &ns, stream);
   if (rc) return rc;
-  if (h->mode != 1) {
+  if (h->acc == nullptr) {
     set_error("nvtb_hashagg_export_packed: the handle is not a sorted accumulator");
     return NVTB_ESTATE;
   }
   *n_host = h->u_known;
   if (out != nullptr && h->u_known > 0)
-    NVTB_CUDA_OK(cudaMemcpyAsync(out, h->acc[h->acc_cur], sizeof(uint64_t) * (size_t)h->u_known,
+    NVTB_CUDA_OK(cudaMemcpyAsync(out, sortacc_pairs(h->acc), sizeof(uint64_t) * (size_t)h->u_known,
                                  cudaMemcpyDeviceToDevice, st));
-  return NVTB_OK;
-}
-
-int nvtb_pairs_lower_bounds(const uint64_t* pairs, int64_t n, const uint32_t* bounds_dev, int m,
-                            int64_t* out_dev, void* stream) {
-  NVTB_REQUIRE(n >= 0 && m >= 0, "negative size");
-  if (m == 0) return NVTB_OK;
-  NVTB_REQUIRE(bounds_dev != nullptr && out_dev != nullptr && (n == 0 || pairs != nullptr), "NULL argument");
-  pairs_lower_bound_kernel<<<(m + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
-      pairs, n, bounds_dev, m, reinterpret_cast<long long*>(out_dev));
-  NVTB_LAUNCH_OK();
-  return NVTB_OK;
-}
-
-// out = merge of two key-sorted, key-unique packed-pair arrays, counts of equal keys added.
-// `out` must hold na + nb pairs; the merged length comes back on the host (one stream sync).
-int nvtb_pairs_merge(const uint64_t* a, int64_t na, const uint64_t* b, int64_t nb, uint64_t* out,
-                     int64_t* n_out_host, void* stream) {
-  NVTB_REQUIRE(na >= 0 && nb >= 0 && n_out_host != nullptr, "bad sizes / NULL n_out");
-  NVTB_REQUIRE(na + nb < (int64_t)0xFFFF0000ll, "more than 2^32 pairs in one merge");
-  cudaStream_t st = (cudaStream_t)stream;
-  *n_out_host = 0;
-  if (na + nb == 0) return NVTB_OK;
-  NVTB_REQUIRE(out != nullptr, "NULL out");
-  if (na == 0 || nb == 0) {
-    NVTB_CUDA_OK(cudaMemcpyAsync(out, na ? a : b, sizeof(uint64_t) * (size_t)(na + nb), cudaMemcpyDeviceToDevice, st));
-    *n_out_host = na + nb;
-    return NVTB_OK;
-  }
-  static bool attrs = false;
-  if (!attrs) {
-    NVTB_CUDA_OK(cudaFuncSetAttribute(merge_write_kernel<true>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MergeSmem)));
-    attrs = true;
-  }
-  const int64_t mt = (na + nb + kMergeTile - 1) / kMergeTile;
-  // scratch: splits[mt + 1] | tile_out[mt] | ub | n_unique | max_count
-  char* scratch = nullptr;
-  const size_t sp_bytes = align_up(sizeof(uint2) * (size_t)(mt + 2), 256);
-  const size_t to_bytes = align_up(sizeof(uint32_t) * (size_t)(mt + 2), 256);
-  NVTB_CUDA_OK(cudaMallocAsync(&scratch, sp_bytes + to_bytes + 256, st));
-  uint2* splits = reinterpret_cast<uint2*>(scratch);
-  uint32_t* tile_out = reinterpret_cast<uint32_t*>(scratch + sp_bytes);
-  uint32_t* ub_dev = reinterpret_cast<uint32_t*>(scratch + sp_bytes + to_bytes);
-  unsigned long long* nu_dev = reinterpret_cast<unsigned long long*>(scratch + sp_bytes + to_bytes + 8);
-  unsigned long long* mx_dev = nu_dev + 1;
-  const uint32_t ub_h = (uint32_t)nb;
-  NVTB_CUDA_OK(cudaMemsetAsync(ub_dev, 0, 64, st));
-  NVTB_CUDA_OK(cudaMemcpyAsync(ub_dev, &ub_h, sizeof(ub_h), cudaMemcpyHostToDevice, st));
-  merge_split_kernel<<<(int)((mt + 1 + 255) / 256), 256, 0, st>>>(a, (uint32_t)na, b, ub_dev, (int)mt, splits);
-  NVTB_LAUNCH_OK();
-  merge_count_kernel<<<(int)mt, kRunThreads, 0, st>>>(a, b, splits, tile_out);
-  NVTB_LAUNCH_OK();
-  scan_tiles_kernel<<<1, kRunThreads, 0, st>>>(tile_out, (int)mt, nullptr, nu_dev);
-  NVTB_LAUNCH_OK();
-  merge_write_kernel<true><<<(int)mt, kRunThreads, sizeof(MergeSmem), st>>>(a, b, splits, tile_out, out, mx_dev);
-  NVTB_LAUNCH_OK();
-  unsigned long long nu_h = 0;
-  NVTB_CUDA_OK(cudaMemcpyAsync(&nu_h, nu_dev, sizeof(nu_h), cudaMemcpyDeviceToHost, st));
-  NVTB_CUDA_OK(cudaFreeAsync(scratch, st));
-  NVTB_CUDA_OK(cudaStreamSynchronize(st));
-  *n_out_host = (int64_t)nu_h;
-  return NVTB_OK;
-}
-
-// contiguous segments of src to their destinations: seg_src[nseg + 1] ascending prefix (device),
-// seg_dst[nseg] (device)
-int nvtb_segment_copy_u64(const uint64_t* src, uint64_t* dst, const int64_t* seg_src_dev, const int64_t* seg_dst_dev,
-                          int nseg, int64_t n, void* stream) {
-  NVTB_REQUIRE(nseg >= 0 && n >= 0, "negative size");
-  if (n == 0 || nseg == 0) return NVTB_OK;
-  NVTB_REQUIRE(src && dst && seg_src_dev && seg_dst_dev, "NULL argument");
-  segment_copy_kernel<<<plain_grid((n + 3) / 4), kThreads, 0, (cudaStream_t)stream>>>(
-      src, dst, reinterpret_cast<const long long*>(seg_src_dev), reinterpret_cast<const long long*>(seg_dst_dev), nseg, n);
-  NVTB_LAUNCH_OK();
   return NVTB_OK;
 }
 
@@ -2052,13 +1669,12 @@ int nvtb_segment_copy_u64(const uint64_t* src, uint64_t* dst, const int64_t* seg
 // wants the cost attributed to the group-by (bench.py) calls it at the end of the last batch.
 int nvtb_hashagg_flush(nvtb_hashagg_t* h, void* stream) {
   NVTB_REQUIRE(h != nullptr, "NULL handle");
-  if (h->mode != 1 || h->stage_rows == 0) return NVTB_OK;
-  return stage_flush(h, (cudaStream_t)stream);
+  return acc_flush(h, (cudaStream_t)stream);
 }
 
 int nvtb_hashagg_mode(nvtb_hashagg_t* h, int* mode_host) {
   NVTB_REQUIRE(h != nullptr && mode_host != nullptr, "NULL argument");
-  *mode_host = h->mode;
+  *mode_host = h->acc != nullptr ? 1 : 0;
   return NVTB_OK;
 }
 

@@ -1,5 +1,5 @@
 // sortagg.cuh — K3 for HIGH-CARDINALITY int32 key columns: a sort-based group-by.
-// Included by hashagg.cu after fold_i32.cuh (uses its partition kernels as the first,
+// Included by sortacc.cu after partition.cuh (its kernels with PartKeyLow are the first,
 // order-free radix pass).
 //
 // Why: once the resident hash table of a column no longer fits the 50 MB L2 (Criteo's
@@ -12,7 +12,7 @@
 //     word = (uint32)(key ^ 2^31) << 32 | (uint32)count        (unsigned order == key order)
 // and a batch is folded in with streaming passes only:
 //     1. LSD radix sort of the batch's valid keys: low 12 bits with the order-free partition
-//        kernels of fold_i32.cuh (shared-memory atomics, nulls dropped and counted on the way),
+//        kernels of partition.cuh (shared-memory atomics, nulls dropped and counted on the way),
 //        bits 12-21 and 22-31 with the stable passes of radix.cuh
 //     2. run-length encode the sorted keys -> (key, first index) per distinct key
 //     3. merge the batch's distinct keys with the accumulator, adding counts (merge-path
@@ -339,53 +339,6 @@ runs_unpack_kernel(const uint64_t* __restrict__ acc, int64_t n, int64_t* __restr
     keys[i] = (int64_t)ukey_to_key(pk_hi(w));
     if (sizes) sizes[i] = (int64_t)pk_lo(w);
   }
-}
-
-// narrow hash table -> packed pairs (unordered); same per-CTA range reservation as export_kernel
-static __global__ void __launch_bounds__(kThreads)
-table_to_pairs_kernel(Table t, uint64_t* __restrict__ out, unsigned long long* cursor,
-                      unsigned long long* max_count) {
-  __shared__ unsigned s_warp[kThreads / 32];
-  __shared__ unsigned long long s_base;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  constexpr int64_t kChunk = (int64_t)kThreads * kExportPerThread;
-  uint32_t mx = 0;
-  for (int64_t c0 = (int64_t)blockIdx.x * kChunk; c0 < t.capacity; c0 += (int64_t)gridDim.x * kChunk) {
-    unsigned long long w[kExportPerThread];
-    unsigned live = 0;
-#pragma unroll
-    for (int j = 0; j < kExportPerThread; ++j) {
-      w[j] = (unsigned long long)t.slots[c0 + (int64_t)j * kThreads + threadIdx.x];
-      if (w[j] != 0ull) live |= 1u << j;
-    }
-    const unsigned mine = __popc(live);
-    unsigned incl = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned y = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += y;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      unsigned tot = 0;
-      for (int q = 0; q < kThreads / 32; ++q) { const unsigned x = s_warp[q]; s_warp[q] = tot; tot += x; }
-      s_base = tot ? atomicAdd(cursor, (unsigned long long)tot) : 0ull;
-    }
-    __syncthreads();
-    int64_t o = (int64_t)s_base + s_warp[warp] + (incl - mine);
-#pragma unroll
-    for (int j = 0; j < kExportPerThread; ++j) {
-      if (!((live >> j) & 1u)) continue;
-      const uint32_t key = (uint32_t)w[j], cnt = (uint32_t)(w[j] >> 32);
-      out[o++] = ((uint64_t)(key ^ 0x80000000u) << 32) | cnt;
-      mx = cnt > mx ? cnt : mx;
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) { const uint32_t y = __shfl_down_sync(0xFFFFFFFFu, mx, o); mx = y > mx ? y : mx; }
-  if (lane == 0 && mx) atomicMax(max_count, (unsigned long long)mx);
 }
 
 // lower bound of every unsigned key bound[j] in the key-sorted packed pairs: out[j] = number of

@@ -21,15 +21,8 @@
 #include <vector>
 
 #include "common.cuh"
+#include "hashagg.cuh"
 #include "radix.cuh"
-
-struct nvtb_hashagg;
-namespace nvtb {
-// hashagg.cu: view of a handle's sorted accumulator (pairs == nullptr: hash table)
-int hashagg_sorted_view(nvtb_hashagg* h, const uint64_t** pairs, int64_t* n_unique, int64_t* null_size,
-                        uint64_t* max_count, int* is_i32_table, cudaStream_t st);
-}
-
 #include "lookup.cuh"
 
 namespace nvtb {
@@ -523,10 +516,6 @@ static int64_t pow2_at_least(int64_t v) {
   int64_t p = 16;
   while (p < v) p <<= 1;
   return p;
-}
-
-static int plain_grid(int64_t n) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>((n + kThreads - 1) / kThreads, (int64_t)sm_count() * 8));
 }
 
 struct VocabScalars {

@@ -81,14 +81,19 @@ def _insert_batches(engine, Column, pack_validity, keys, valid, cuts, agg=None):
 
 @pytest.mark.parametrize("card,n", [(50_000_000, 2_000_000), (300_000, 1_500_000), (7, 600_000)])
 @pytest.mark.parametrize("with_nulls", [False, True])
-def test_sorted_accumulator_counts(monkeypatch, card, n, with_nulls):
-    """every batch radix-sorted, run-length encoded and merged: exact value_counts incl. nulls"""
+@pytest.mark.parametrize("ragged", [False, True])
+def test_sorted_accumulator_counts(monkeypatch, card, n, with_nulls, ragged):
+    """every batch grouped and merged: exact value_counts incl. nulls.  ragged: the first batch is not
+    a multiple of 8 rows long, so the batch after it bypasses the staging buffer (the staged rows are
+    flushed and it goes in on its own)."""
     engine, Column, pack_validity = _engine()
     monkeypatch.setenv("NVTB_RUNS_MIN_KEYS", "1")
     g = torch.Generator(device="cuda").manual_seed(card % 1000 + n % 97)
     keys = (torch.randint(0, card, (n,), generator=g, device="cuda", dtype=torch.int64) * 2654435761 % (2**32) - 2**31).to(torch.int32)
     valid = (torch.rand(n, generator=g, device="cuda") > 0.07) if with_nulls else None
     cuts = [0, 64 * 4000, 64 * 4000 + 64 * 9001, n]              # three uneven batches (64-row aligned cuts)
+    if ragged:
+        cuts = [0, 64 * 4000 + 3, 64 * 4000 + 64 * 9001, n]
     agg = _insert_batches(engine, Column, pack_validity, keys, valid, cuts)
     assert agg.mode == 1
     k, s, _, null_size, _ = agg.export()
@@ -178,15 +183,21 @@ def test_vocab_from_sorted_accumulator(monkeypatch, cut):
 
 
 @pytest.mark.parametrize("shape", ["uniform32", "dense_small_range", "heavy_hitters", "cluster_fallback"])
-def test_bucket_groupby_paths_agree(monkeypatch, shape):
+@pytest.mark.parametrize("stage_rows", [None, 64 * 20000, 0])
+def test_bucket_groupby_paths_agree(monkeypatch, shape, stage_rows):
     """The staged batches of a sorted accumulator are grouped by ONE range partition + direct-address
     counting in shared memory (csrc/bucketagg.cuh); the radix pipeline (NVTB_SORT_PATH=radix) is the
     fallback when a window holds more duplicated values than the counters a CTA has.  Both must give
     torch.unique's answer for: keys over the whole int32 range; a dense small range (the window
     shrinks to a few values); a few values with millions of rows each; and a dense cluster inside a
-    wide range (more than 14 336 duplicated values in one 2^18 window: the fallback fires)."""
+    wide range (more than 14 336 duplicated values in one 2^18 window: the fallback fires).
+    stage_rows: one flush per fit (None); a stage smaller than the fit (64 * 20000: the second batch
+    flushes the first, the third flushes the second into a non-empty accumulator and then goes in
+    on its own); or no staging, one group-by + merge per batch (0)."""
     engine, Column, pack_validity = _engine()
     monkeypatch.setenv("NVTB_RUNS_MIN_KEYS", "1")
+    if stage_rows is not None:
+        monkeypatch.setenv("NVTB_STAGE_ROWS", str(stage_rows))
     n = 4_000_000
     g = torch.Generator(device="cuda").manual_seed(len(shape))
     if shape == "uniform32":
@@ -231,3 +242,36 @@ def test_small_staging_buffer_merges_flushes(monkeypatch):
     k, s, _, null_size, _ = agg.export()
     u, c = _ref_counts(keys, valid)
     assert torch.equal(k, u) and torch.equal(s, c) and null_size == int((~valid).sum())
+
+
+def _unique_packed(g, n, lo, hi):
+    """n distinct int32 keys in [lo, hi) with counts in [1, 1000], as key-ordered packed pairs"""
+    keys = torch.unique(torch.randint(lo, hi, (n,), generator=g, device="cuda", dtype=torch.int64))
+    counts = torch.randint(1, 1001, (keys.numel(),), generator=g, device="cuda", dtype=torch.int64)
+    return keys, counts, ((keys + 2**31) << 32) | counts
+
+
+@pytest.mark.parametrize("case", ["a_empty", "b_empty", "disjoint", "identical", "overlap"])
+def test_pairs_merge(case):
+    """nvtb_pairs_merge (the cross-GPU shard merge) against a torch reference: the merged pairs stay
+    key-ordered and key-unique, and the counts of a key present on both sides are added"""
+    engine, _, _ = _engine()
+    g = torch.Generator(device="cuda").manual_seed(len(case))
+    if case == "disjoint":
+        ka, ca, a = _unique_packed(g, 30_000, -2**31, 0)
+        kb, cb, b = _unique_packed(g, 20_000, 0, 2**31 - 1)
+    elif case == "identical":
+        ka, ca, a = _unique_packed(g, 50_000, -2**31, 2**31 - 1)
+        kb, cb, b = ka, ca * 3, ((ka + 2**31) << 32) | (ca * 3)
+    else:   # overlap: far more than one 4096-element merge tile, keys drawn from a shared range
+        ka, ca, a = _unique_packed(g, 700_000, -3_000_000, 3_000_000)
+        kb, cb, b = _unique_packed(g, 500_000, -3_000_000, 3_000_000)
+    if case == "a_empty":
+        ka, ca, a = ka[:0], ca[:0], a[:0]
+    elif case == "b_empty":
+        kb, cb, b = kb[:0], cb[:0], b[:0]
+    got = engine.pairs_merge(a.contiguous(), b.contiguous())
+    k = torch.cat([ka, kb])
+    u, inv = torch.unique(k, return_inverse=True)
+    c = torch.zeros_like(u).index_add_(0, inv, torch.cat([ca, cb]))
+    assert torch.equal(got, ((u + 2**31) << 32) | c)
