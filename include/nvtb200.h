@@ -541,6 +541,46 @@ int nvtb_lag_same_key(const nvtb_col_t* keys, int n_keys, int64_t n, int64_t shi
 int nvtb_difference_lag(const nvtb_col_t* cols, int ncols, int64_t n, int64_t shift, const uint8_t* same,
                         float* const* outs, uint8_t* const* out_valids, void* stream);
 
+/* ---- row selection: Filter and Dropna (csrc/filter.cu, K11) ---------------------------------
+ * A mask is a bitmask in the validity layout: bit (i & 7) of byte (i >> 3) is row i, and it is
+ * padded to whole 32-byte blocks like pack_validity: ((ceil(n / 8) + 31) / 32) * 32 bytes.  The
+ * mask writers fill every byte of that padding and leave the bits at rows >= n zero.  Every entry
+ * point returns NVTB_OK for n = 0 without touching its outputs. */
+typedef enum {
+  NVTB_CMP_EQ = 0,
+  NVTB_CMP_NE = 1,
+  NVTB_CMP_LT = 2,
+  NVTB_CMP_LE = 3,
+  NVTB_CMP_GT = 4,
+  NVTB_CMP_GE = 5
+} nvtb_cmp_op_t;
+typedef enum { NVTB_MASK_AND = 0, NVTB_MASK_OR = 1, NVTB_MASK_XOR = 2, NVTB_MASK_NOT = 3 } nvtb_mask_op_t;
+/* nvtb_mask_compare (reference nvtabular/ops/filter.py:51-55, the comparisons f(df) makes, i.e.
+ * pandas `df[c] op x`): bit i = a[i] op (b ? b[i] : scalar).  Both operands are converted to
+ * cmp_type (NVTB_I64, NVTB_F32 or NVTB_F64; I64 only when neither operand is a float), and
+ * scalar_bits is the scalar's bit pattern in cmp_type (low bytes).  A null operand, like a NaN,
+ * gives true for NVTB_CMP_NE and false for every other op.  a and b: int32, int64, float32,
+ * float64 or uint8 columns of n rows. */
+int nvtb_mask_compare(const nvtb_col_t* a, const nvtb_col_t* b, int op, int cmp_type, uint64_t scalar_bits,
+                      int64_t n, uint8_t* mask_out, void* stream);
+/* nvtb_mask_notnull (reference nvtabular/ops/dropna.py:33-37, df.dropna(subset=cols); pandas
+ * notnull): bit i is set when each of the ncols (<= 16) columns is valid at row i and, if it is a
+ * float, not NaN there. */
+int nvtb_mask_notnull(const nvtb_col_t* cols, int ncols, int64_t n, uint8_t* mask_out, void* stream);
+/* nvtb_mask_logic (filter.py:51-55, pandas & | ^ ~ of bool Series): out = a op b, or ~a for
+ * NVTB_MASK_NOT (b unused).  Masks 16-byte aligned; out aliases neither input. */
+int nvtb_mask_logic(const uint8_t* a, const uint8_t* b, int64_t n, int op, uint8_t* out, void* stream);
+/* nvtb_mask_count (filter.py:56-60 and dropna.py:35, the length of the indexed frame): tile_off
+ * (ceil(n / 2048) + 1 int64, 32-byte aligned) receives the exclusive scan of the set bits of every
+ * 2048-row tile and *n_kept_host their total.  Bits at rows >= n are ignored.  Mask 8-byte
+ * aligned.  Synchronises the stream. */
+int nvtb_mask_count(const uint8_t* mask, int64_t n, int64_t* tile_off, int64_t* n_kept_host, void* stream);
+/* nvtb_mask_select (pandas boolean indexing, df[mask], then reset_index(drop=True)): rows_out
+ * (n_kept int64) receives the rows whose bit is set, in ascending order, from nvtb_mask_count's
+ * tile_off.  No atomics: the output is deterministic.  Moving the columns to those rows is
+ * nvtb_join_gather (fixed width) and nvtb_gb_list_rows (lists). */
+int nvtb_mask_select(const uint8_t* mask, int64_t n, const int64_t* tile_off, int64_t* rows_out, void* stream);
+
 /* ---- external-table join: JoinExternal operator (csrc/join.cu, K9) -------------------------
  * Replaces, per partition, reference nvtabular/ops/join_external.py:148-164: df.merge(ext,
  * left_on=on, right_on=on_ext, how=how) followed by sort_values("__tmp__") back to row order.

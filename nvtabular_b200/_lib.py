@@ -130,6 +130,12 @@ _SIGNATURES = {
     "nvtb_lag_same_key": (c_int, [POINTER(nvtb_col_t), c_int, c_int64, c_int64, c_void_p, c_void_p]),
     "nvtb_difference_lag": (c_int, [POINTER(nvtb_col_t), c_int, c_int64, c_int64, c_void_p, POINTER(c_void_p),
                                     POINTER(c_void_p), c_void_p]),
+    "nvtb_mask_compare": (c_int, [POINTER(nvtb_col_t), POINTER(nvtb_col_t), c_int, c_int, c_uint64, c_int64, c_void_p,
+                                  c_void_p]),
+    "nvtb_mask_notnull": (c_int, [POINTER(nvtb_col_t), c_int, c_int64, c_void_p, c_void_p]),
+    "nvtb_mask_logic": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
+    "nvtb_mask_count": (c_int, [c_void_p, c_int64, c_void_p, POINTER(c_int64), c_void_p]),
+    "nvtb_mask_select": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -958,3 +958,86 @@ def join_gather(cols: Sequence[Column], rows: torch.Tensor, masked: Sequence[boo
                                                             for v in valids[s:e]]), _lib.stream_ptr()))
         _count()
     return [Column(o[:m], v, None, c.dictionary, None, c.is_bool) for o, v, c in zip(outs, valids, cols)]
+
+
+def take_rows(cols, rows: torch.Tensor, masked: bool = False):
+    """{name: Column} at int64 `rows`, in the same order; a fixed-width column through
+    nvtb_join_gather, a list column through nvtb_gb_list_rows over its gathered offsets.  With
+    `masked`, row -1 is null (an empty list for a list column)."""
+    flat = [n for n, c in cols.items() if not c.is_list]
+    res = dict(zip(flat, join_gather([cols[n] for n in flat], rows, [masked] * len(flat)))) if flat else {}
+    for n, c in cols.items():
+        if c.is_list:
+            lo, hi = join_gather([Column(c.offsets[:-1]), Column(c.offsets[1:])], rows, [False, False])
+            res[n] = gb_list_rows(c.leaves(), lo.data, hi.data)
+    return {n: res[n] for n in cols}
+
+
+# ------------------------------------------------------------- row selection (K11, csrc/filter.cu)
+CMP_EQ, CMP_NE, CMP_LT, CMP_LE, CMP_GT, CMP_GE = range(6)    # nvtb_cmp_op_t
+MASK_AND, MASK_OR, MASK_XOR, MASK_NOT = range(4)            # nvtb_mask_op_t
+NOTNULL_MAX_COLS = 16   # columns of one nvtb_mask_notnull launch (kMaxNotnullCols, csrc/filter.cu)
+MASK_TILE = 2048        # rows per tile of nvtb_mask_count / nvtb_mask_select (kScanTile, csrc/scan.cuh)
+
+
+def mask_nbytes(n: int) -> int:
+    """bytes of a row mask of n rows: pack_validity's padding, which the mask kernels fill"""
+    return (((n + 7) // 8 + 31) // 32) * 32
+
+
+def mask_compare(a: Column, b: Optional[Column], op: int, cmp_type: int, scalar_bits: int, n: int) -> torch.Tensor:
+    """row mask of a op (b, or the scalar whose bit pattern in cmp_type is scalar_bits); a null
+    operand is true for CMP_NE only (nvtb_mask_compare)"""
+    lib = _lib.load()
+    out = torch.empty(mask_nbytes(n), dtype=torch.uint8, device=a.data.device)
+    with _timed("mask", _in_bytes([a] if b is None else [a, b]) + n / 8.0):
+        _lib.check(lib.nvtb_mask_compare(_descs([a]), _descs([b]) if b is not None else None, int(op), int(cmp_type),
+                                         int(scalar_bits), n, _ptr(out), _lib.stream_ptr()))
+    _count()
+    return out
+
+
+def mask_logic(a: torch.Tensor, b: Optional[torch.Tensor], n: int, op: int) -> torch.Tensor:
+    """a & b, a | b, a ^ b or ~a of two row masks of n rows (nvtb_mask_logic)"""
+    lib = _lib.load()
+    out = torch.empty_like(a)
+    with _timed("mask", n / 8.0 * (2 if b is None else 3)):
+        _lib.check(lib.nvtb_mask_logic(_ptr(a), _ptr(b), n, int(op), _ptr(out), _lib.stream_ptr()))
+    _count()
+    return out
+
+
+def mask_notnull(cols: Sequence[Column], n: int) -> torch.Tensor:
+    """row mask: every column valid and, if a float, not NaN (nvtb_mask_notnull; more than
+    NOTNULL_MAX_COLS columns are ANDed)"""
+    lib = _lib.load()
+    out = None
+    for s in range(0, len(cols), NOTNULL_MAX_COLS):
+        part = cols[s:s + NOTNULL_MAX_COLS]
+        m = torch.empty(mask_nbytes(n), dtype=torch.uint8, device=part[0].data.device)
+        with _timed("mask", _in_bytes(part) + n / 8.0):
+            _lib.check(lib.nvtb_mask_notnull(_descs(part), len(part), n, _ptr(m), _lib.stream_ptr()))
+        _count()
+        out = m if out is None else mask_logic(out, m, n, MASK_AND)
+    return out
+
+
+def mask_count(mask: torch.Tensor, n: int):
+    """-> (kept rows, tile offsets for mask_select); one host read (nvtb_mask_count)"""
+    lib = _lib.load()
+    tile_off = torch.empty((n + MASK_TILE - 1) // MASK_TILE + 1, dtype=torch.int64, device=mask.device)
+    kept = c_int64(0)
+    with _timed("count", n / 8.0 + tile_off.numel() * 16.0):
+        _lib.check(lib.nvtb_mask_count(_ptr(mask), n, _ptr(tile_off), byref(kept), _lib.stream_ptr()))
+    _count(4 if n else 0)
+    return kept.value, tile_off
+
+
+def mask_select(mask: torch.Tensor, n: int, tile_off: torch.Tensor, n_kept: int) -> torch.Tensor:
+    """the int64 ids of the n_kept rows whose bit is set, ascending (nvtb_mask_select)"""
+    lib = _lib.load()
+    rows = torch.empty(max(n_kept, 1), dtype=torch.int64, device=mask.device)
+    with _timed("select", n / 8.0 + tile_off.numel() * 8.0 + n_kept * 8.0):
+        _lib.check(lib.nvtb_mask_select(_ptr(mask), n, _ptr(tile_off), _ptr(rows), _lib.stream_ptr()))
+    _count()
+    return rows[:n_kept]

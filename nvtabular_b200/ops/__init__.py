@@ -4,7 +4,9 @@ from .base import Operator, StatOperator  # noqa: F401
 from .categorify import Categorify  # noqa: F401
 from .clip_log import Clip, LogOp  # noqa: F401
 from .difference_lag import DifferenceLag  # noqa: F401
+from .dropna import Dropna  # noqa: F401
 from .fill import FillMissing  # noqa: F401
+from .filter import Filter  # noqa: F401
 from .groupby import Groupby  # noqa: F401
 from .hash_bucket import HashBucket, emb_sz_rule  # noqa: F401
 from .join_external import JoinExternal  # noqa: F401

@@ -338,22 +338,11 @@ class JoinExternal(Operator):
             # unique ext keys: exactly one output row per left row, in order
             ext_rows, _, _ = t.join.probe(key, "left", scan=False)
             out = dict(left)
-            out.update(_take(ext_cols, ext_rows, masked=True))
+            out.update(engine.take_rows(ext_cols, ext_rows, masked=True))
         else:
             first, off, n_out = t.join.probe(key, self.how, scan=True)
             left_rows, ext_rows = t.join.expand(first, off, n_out)
-            out = _take(left, left_rows, masked=False)
-            out.update(_take(ext_cols, ext_rows, masked=self.how == "left"))
+            out = engine.take_rows(left, left_rows)
+            out.update(engine.take_rows(ext_cols, ext_rows, masked=self.how == "left"))
         return DeviceFrame({n: out[n] for n in self.column_mapping(col_selector)})
 
-
-def _take(cols: Dict[str, Column], rows: torch.Tensor, masked: bool) -> Dict[str, Column]:
-    """every column at `rows` (-1 = null; an empty list for a list column)"""
-    flat = [n for n, c in cols.items() if not c.is_list]
-    lists = [n for n, c in cols.items() if c.is_list]
-    res = dict(zip(flat, engine.join_gather([cols[n] for n in flat], rows, [masked] * len(flat)))) if flat else {}
-    for n in lists:
-        c = cols[n]
-        lo, hi = engine.join_gather([Column(c.offsets[:-1]), Column(c.offsets[1:])], rows, [False, False])
-        res[n] = engine.gb_list_rows(c.leaves(), lo.data, hi.data)
-    return res

@@ -220,6 +220,28 @@ def _target_encoding_from(params, state, adir):
     return op
 
 
+def _callable_to_dict(f):
+    """a module-level function as {"module", "qualname"} (reference graph_serializer.py:71-99)"""
+    if getattr(f, "__name__", None) == "<lambda>":
+        raise WorkflowSerializationError(
+            f"Cannot serialize {f!r}: a lambda has no importable name. Define the function with `def` "
+            "in a module that can be imported where the workflow is loaded, and pass that function.")
+    if getattr(f, "__module__", None) == "__main__":
+        raise WorkflowSerializationError(
+            f"Cannot serialize '{f.__qualname__}': it is defined in __main__. Move it to an importable module.")
+    if getattr(f, "__module__", None) is None or "<locals>" in getattr(f, "__qualname__", "<locals>"):
+        raise WorkflowSerializationError(f"Cannot serialize {f!r}: it has no importable module and name")
+    return {"module": f.__module__, "qualname": f.__qualname__}
+
+
+def _callable_from_dict(d):
+    import importlib
+    obj = importlib.import_module(d["module"])
+    for part in d["qualname"].split("."):
+        obj = getattr(obj, part)
+    return obj
+
+
 def _registry():
     from . import ops
     return {
@@ -252,6 +274,10 @@ def _registry():
                                               "pad_value": op.pad_value}, {}),
             lambda p, s, adir: ops.ListSlice(start=p["start"], end=p.get("end"), pad=p.get("pad", False),
                                              pad_value=p.get("pad_value", 0.0))),
+        "nvtabular.ops.dropna.Dropna": (ops.Dropna, lambda op, adir: ({}, {}), lambda p, s, adir: ops.Dropna()),
+        "nvtabular.ops.filter.Filter": (
+            ops.Filter, lambda op, adir: ({"f": _callable_to_dict(op.f)}, {}),
+            lambda p, s, adir: ops.Filter(f=_callable_from_dict(p["f"]))),
     }
 
 

@@ -24,6 +24,24 @@ from .ops.base import Operator, StatOperator
 from .ops.fill import materialize_many
 
 
+def _merge(frames: List[DeviceFrame]) -> DeviceFrame:
+    """the columns of every frame in one frame (a later frame's column replaces an earlier one of the
+    same name).  Frames of different lengths raise ValueError: rows would be misaligned, which the
+    reference does silently, e.g. for a Filter / Dropna branch added to an unfiltered one."""
+    out = DeviceFrame()
+    lengths = []
+    for f in frames:
+        for k, v in f.items():
+            out[k] = v
+        if f.columns:
+            lengths.append((len(f), f.columns))
+    if len({n for n, _ in lengths}) > 1:
+        sides = "; ".join(f"{cols} have {n} rows" for n, cols in lengths)
+        raise ValueError(f"cannot merge frames with different row counts ({sides}): a Filter, Dropna, Groupby "
+                         "or inner JoinExternal branch cannot be combined with a branch of other rows")
+    return out
+
+
 def _execute_node(node: Node, root: DeviceFrame, cache: Dict[int, DeviceFrame]) -> DeviceFrame:
     hit = cache.get(id(node))
     if hit is not None:
@@ -36,19 +54,13 @@ def _execute_node(node: Node, root: DeviceFrame, cache: Dict[int, DeviceFrame]) 
     else:
         frames = [_execute_node(p, root, cache) for p in node.upstream]
         if node.kind in ("concat",):
-            out = DeviceFrame()
-            for f in frames:
-                for k, v in f.items():
-                    out[k] = v
+            out = _merge(frames)
         elif node.kind == "subtract":
             out = frames[0].drop(node.selector.names)
         elif node.kind == "subset":
             out = frames[0][node.selector.names]
         else:
-            inp = DeviceFrame()
-            for f in frames:
-                for k, v in f.items():
-                    inp[k] = v
+            inp = _merge(frames)
             if not node.op.fuses_fill:
                 names = inp.columns
                 cols = materialize_many([inp[n] for n in names])
@@ -102,11 +114,7 @@ class _UpstreamPartitions:
     def __iter__(self):
         for part in self.dataset.partitions():
             cache: Dict[int, DeviceFrame] = {}
-            out = DeviceFrame()
-            for up in self.node.upstream:
-                for k, v in _execute_node(up, part, cache).items():
-                    out[k] = v
-            yield out
+            yield _merge([_execute_node(up, part, cache) for up in self.node.upstream])
 
 
 class Workflow:
