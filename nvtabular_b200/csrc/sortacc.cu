@@ -17,7 +17,10 @@ struct SortedAcc {
   uint64_t* acc[2] = {nullptr, nullptr};   // acc[cur] holds the u pairs, the other one takes the next merge
   int64_t acc_cap[2] = {0, 0};
   int cur = 0;
-  uint32_t* d_n = nullptr;   // device uint32[4]: [1] valid keys of the batch, [2] distinct keys of the batch
+  // device uint32[8] of the batch being grouped: [1] valid keys, [2] distinct keys, [3] the most
+  // rows of a bucket, [4] min and [5] max of u = key ^ 2^31 over the valid keys (folded by the
+  // staging copies), [6] lo, [7] shift of the bucket partition.  [2, 8) is read back in one copy.
+  uint32_t* d_n = nullptr;
   // staging: batches are only COPIED (keys + validity bytes) until NVTB_STAGE_ROWS rows are
   // waiting or somebody reads the handle; one group-by + merge then takes all of them (a merge
   // per batch re-reads and re-writes the whole accumulator, so its cost grows with every batch)
@@ -111,17 +114,28 @@ static int merge_pairs(const uint64_t* A, int64_t ua, const uint64_t* B, const u
   return NVTB_OK;
 }
 
+constexpr int kDnWords = 8;
+
+// d_n[4, 6) = {~0, 0}: no valid key seen yet
+static int minmax_reset(SortedAcc* a, cudaStream_t st) {
+  NVTB_CUDA_OK(cudaMemsetAsync(a->d_n + 4, 0xFF, sizeof(uint32_t), st));
+  NVTB_CUDA_OK(cudaMemsetAsync(a->d_n + 5, 0, sizeof(uint32_t), st));
+  return NVTB_OK;
+}
+
 // bucket route (bucketagg.cuh): range partition + direct-address counting, no sort.  The batch's
-// pairs go to acc[other] when the accumulator is empty, else to c.rle.  *ok = false: some window
+// pairs go to acc[other] when the accumulator is empty, else to c.rle.  have_minmax: the staging
+// copies have folded the batch's min / max into d_n[4, 6) already.  *ok = false: some window
 // holds more than kBkDupCap duplicated values and the radix route has to redo the batch (the
 // nulls are counted already).
 static int bucket_route(SortedAcc* a, const int32_t* kp, const uint8_t* mp, int64_t m, int64_t ua, Counters* ctr,
-                        const SortCarve& c, cudaStream_t st, bool* ok) {
+                        bool have_minmax, const SortCarve& c, cudaStream_t st, bool* ok) {
   static bool attrs = false;
-  constexpr int kBkScatterSmem = kPartTile * 4 + 2 * 4 * kBkParts;
+  constexpr int kBkScatterSmem = kPartTile * 4 + 2 * 4 * kBkCoarse;
   if (!attrs) {
     NVTB_CUDA_OK(cudaFuncSetAttribute(part_hist_kernel<PartRange>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kBkParts));
-    NVTB_CUDA_OK(cudaFuncSetAttribute(part_scatter_kernel<PartRange>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBkScatterSmem));
+    NVTB_CUDA_OK(cudaFuncSetAttribute(part_scatter_kernel<PartRangeCoarse>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      kBkScatterSmem));
     NVTB_CUDA_OK(cudaFuncSetAttribute(bk_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kBkCountSmem));
     NVTB_CUDA_OK(cudaFuncSetAttribute(bk_emit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kBkEmitSmem));
     attrs = true;
@@ -134,40 +148,56 @@ static int bucket_route(SortedAcc* a, const int32_t* kp, const uint8_t* mp, int6
   uint32_t* total = c.part_meta;                    // -> exclusive starts after the scan
   uint32_t* cursor = c.part_meta + kBkParts;
   uint32_t* distinct = c.part_meta + 2 * kBkParts;  // -> output offsets after the scan
-  uint32_t* mm = c.part_meta + 4 * kBkParts;        // {min, max}
-  uint32_t* par = mm + 2;                           // {lo, shift}
-  unsigned int* flag = reinterpret_cast<unsigned int*>(mm + 4);
-  const uint32_t mm_init[6] = {0xFFFFFFFFu, 0u, 0u, 0u, 0u, 0u};
-  NVTB_CUDA_OK(cudaMemcpyAsync(mm, mm_init, sizeof(mm_init), cudaMemcpyHostToDevice, st));
+  uint32_t* coarse = c.part_meta + 3 * kBkParts;    // cursors of the 512 coarse ranges
+  unsigned int* flag = reinterpret_cast<unsigned int*>(c.part_meta + 4 * kBkParts);
+  uint32_t* max_rows = a->d_n + 3;
+  uint32_t* mm = a->d_n + 4;                        // {min, max}
+  uint32_t* par = a->d_n + 6;                       // {lo, shift}
+  NVTB_CUDA_OK(cudaMemsetAsync(flag, 0, sizeof(unsigned int), st));
+  NVTB_CUDA_OK(cudaMemsetAsync(max_rows, 0, sizeof(uint32_t), st));
   NVTB_CUDA_OK(cudaMemsetAsync(total, 0, sizeof(uint32_t) * kBkParts, st));
-  bk_minmax_kernel<<<(int)std::min<int64_t>(tiles, 4 * sms), kPartThreads, 0, st>>>(kp, mp, m, mm, aligned);
-  NVTB_LAUNCH_OK();
+  if (!have_minmax) {
+    int rc = minmax_reset(a, st);
+    if (rc) return rc;
+    bk_minmax_kernel<<<(int)std::min<int64_t>(tiles, 4 * sms), kPartThreads, 0, st>>>(kp, mp, m, mm, aligned);
+    NVTB_LAUNCH_OK();
+  }
   bk_params_kernel<<<1, 1, 0, st>>>(mm, par);
   NVTB_LAUNCH_OK();
-  const PartRange pol{kBkLgParts, par};
   part_hist_kernel<PartRange><<<(int)std::min<int64_t>(tiles, 3 * sms), kPartThreads, 4 * kBkParts, st>>>(
-      kp, mp, m, pol, total, ctr, aligned);
+      kp, mp, m, PartRange{kBkLgParts, par}, total, ctr, aligned);
   NVTB_LAUNCH_OK();
   scan_tiles_kernel<<<1, kRunThreads, 0, st>>>(total, kBkParts, n_valid, nullptr);
   NVTB_LAUNCH_OK();
-  NVTB_CUDA_OK(cudaMemcpyAsync(cursor, total, sizeof(uint32_t) * kBkParts, cudaMemcpyDeviceToDevice, st));
-  part_scatter_kernel<PartRange><<<(int)std::min<int64_t>(tiles, sms), kPartThreads, kBkScatterSmem, st>>>(
-      kp, mp, m, pol, cursor, reinterpret_cast<int32_t*>(c.keys_a), aligned);
+  // two-level partition: 512 coarse ranges (runs of ~32 keys per tile and range) into keys_b, then
+  // each range into its 16 buckets (runs of hundreds of keys) at their final place in keys_a; the
+  // single pass into 8192 buckets wrote runs of ~2 keys, a few bytes of a sector at a time
+  bk_cursors_kernel<<<kBkParts / 256, 256, 0, st>>>(total, cursor, coarse);
   NVTB_LAUNCH_OK();
-  bk_count_kernel<<<kBkParts, kBkThreads, kBkCountSmem, st>>>(c.keys_a, total, n_valid, par, distinct);
+  part_scatter_kernel<PartRangeCoarse><<<(int)std::min<int64_t>(tiles, 2 * sms), kPartThreads, kBkScatterSmem, st>>>(
+      kp, mp, m, PartRangeCoarse{kBkLgParts - kBkLgFine, par}, coarse, reinterpret_cast<int32_t*>(c.keys_b), aligned);
+  NVTB_LAUNCH_OK();
+  bk_refine_kernel<<<(int)std::min<int64_t>(m / kBkRefineTile + kBkCoarse, 2 * sms), kPartThreads, 0, st>>>(
+      c.keys_b, total, n_valid, par, cursor, c.keys_a);
+  NVTB_LAUNCH_OK();
+  bk_count_kernel<<<kBkParts, kBkThreads, kBkCountSmem, st>>>(c.keys_a, total, n_valid, par, distinct, max_rows);
   NVTB_LAUNCH_OK();
   scan_tiles_kernel<<<1, kRunThreads, 0, st>>>(distinct, kBkParts, n_batch, ua == 0 ? &ctr->n_unique : nullptr);
   NVTB_LAUNCH_OK();
   // the accumulator is sized for what the batch really holds (its distinct keys are known now),
-  // not for the worst case of all rows distinct
-  uint32_t nb_h = 0;
-  NVTB_CUDA_OK(cudaMemcpyAsync(&nb_h, n_batch, sizeof(nb_h), cudaMemcpyDeviceToHost, st));
+  // not for the worst case of all rows distinct; the emit's shared memory for the batch's window
+  // and for at most half the rows of its fullest bucket as counters (a duplicated value takes two
+  // rows), not for the widest window: two CTAs per SM fit up to shift 18
+  uint32_t h[kDnWords - 2];          // d_n[2, 8)
+  NVTB_CUDA_OK(cudaMemcpyAsync(h, n_batch, sizeof(h), cudaMemcpyDeviceToHost, st));
   NVTB_CUDA_OK(cudaStreamSynchronize(st));
+  const uint32_t nb_h = h[0], shift_h = h[5];
+  const int cap = (int)std::min<uint32_t>((uint32_t)kBkDupCap, h[1] / 2);
   int rc = acc_reserve(a, a->cur ^ 1, ua + (int64_t)nb_h, st);
   if (rc) return rc;
   uint64_t* B = (ua == 0) ? a->acc[a->cur ^ 1] : c.rle;
-  bk_emit_kernel<<<kBkParts, kBkThreads, kBkEmitSmem, st>>>(c.keys_a, total, n_valid, par, distinct, B, flag,
-                                                             &ctr->max_count);
+  bk_emit_kernel<<<kBkParts, kBkThreads, bk_emit_smem(shift_h, cap), st>>>(c.keys_a, total, n_valid, par, distinct,
+                                                                            B, (uint32_t)cap, flag, &ctr->max_count);
   NVTB_LAUNCH_OK();
   unsigned int flag_h = 0;
   NVTB_CUDA_OK(cudaMemcpyAsync(&flag_h, flag, sizeof(flag_h), cudaMemcpyDeviceToHost, st));
@@ -219,9 +249,9 @@ static int radix_route(SortedAcc* a, const int32_t* kp, const uint8_t* mp, int64
   return NVTB_OK;
 }
 
-// fold m rows of int32 keys into the accumulator, which holds ua pairs
-int sortacc_insert(SortedAcc* a, const int32_t* kp, const uint8_t* mp, int64_t m, int64_t ua, Counters* ctr,
-                   cudaStream_t st) {
+// fold m rows of int32 keys into the accumulator, which holds ua pairs (have_minmax: see bucket_route)
+static int insert_rows(SortedAcc* a, const int32_t* kp, const uint8_t* mp, int64_t m, int64_t ua, Counters* ctr,
+                       bool have_minmax, cudaStream_t st) {
   const int64_t mt = (ua + m + kMergeTile - 1) / kMergeTile;
   SortCarve c;
   int rc = sort_scratch_acquire(m, 64, mt, st, &c);
@@ -230,7 +260,7 @@ int sortacc_insert(SortedAcc* a, const int32_t* kp, const uint8_t* mp, int64_t m
   const bool radix_only = path_env && strcmp(path_env, "radix") == 0;
   bool bucketed = false;
   if (!radix_only) {
-    rc = bucket_route(a, kp, mp, m, ua, ctr, c, st, &bucketed);
+    rc = bucket_route(a, kp, mp, m, ua, ctr, have_minmax, c, st, &bucketed);
     if (rc) return rc;
   }
   if (!bucketed) {
@@ -249,6 +279,11 @@ int sortacc_insert(SortedAcc* a, const int32_t* kp, const uint8_t* mp, int64_t m
   return g_sort.release(st);
 }
 
+int sortacc_insert(SortedAcc* a, const int32_t* kp, const uint8_t* mp, int64_t m, int64_t ua, Counters* ctr,
+                   cudaStream_t st) {
+  return insert_rows(a, kp, mp, m, ua, ctr, false, st);
+}
+
 // rows a sorted accumulator stages before it sorts (NVTB_STAGE_ROWS, default 2^28 = 1 GiB of keys)
 static int64_t stage_cap_rows() {
   const char* e = getenv("NVTB_STAGE_ROWS");
@@ -263,8 +298,8 @@ int sortacc_create(SortedAcc** out, int64_t u, cudaStream_t st, uint64_t** pairs
   NVTB_REQUIRE(a != nullptr, "host allocation failed");
   *out = a;
   *pairs = nullptr;
-  NVTB_CUDA_OK(cudaMalloc(&a->d_n, sizeof(uint32_t) * 4));
-  NVTB_CUDA_OK(cudaMemsetAsync(a->d_n, 0, sizeof(uint32_t) * 4, st));
+  NVTB_CUDA_OK(cudaMalloc(&a->d_n, sizeof(uint32_t) * kDnWords));
+  NVTB_CUDA_OK(cudaMemsetAsync(a->d_n, 0, sizeof(uint32_t) * kDnWords, st));
   if (u > 0) {
     int rc = acc_reserve(a, 0, u, st);
     if (rc) return rc;
@@ -319,11 +354,15 @@ int sortacc_stage(SortedAcc* a, const int32_t* kp, const uint8_t* mp, int64_t m,
     NVTB_CUDA_OK(cudaMallocAsync(&a->stage_mask, (size_t)(want / 8 + 64), st));
     a->stage_cap = want;
   }
-  NVTB_CUDA_OK(cudaMemcpyAsync(a->stage_keys + a->stage_rows, kp, sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToDevice, st));
-  uint8_t* md = a->stage_mask + (a->stage_rows >> 3);
-  const size_t mbytes = (size_t)((m + 7) >> 3);
-  if (mp) NVTB_CUDA_OK(cudaMemcpyAsync(md, mp, mbytes, cudaMemcpyDeviceToDevice, st));
-  else    NVTB_CUDA_OK(cudaMemsetAsync(md, 0xFF, mbytes, st));
+  if (a->stage_rows == 0) {
+    int rc = minmax_reset(a, st);
+    if (rc) return rc;
+  }
+  const int64_t tiles = (m + kPartTile - 1) / kPartTile;
+  bk_stage_kernel<<<(int)std::min<int64_t>(tiles, 4 * sm_count()), kPartThreads, 0, st>>>(
+      kp, mp, m, a->stage_keys + a->stage_rows, a->stage_mask + (a->stage_rows >> 3), a->d_n + 4,
+      is_aligned32(kp) ? 1 : 0);
+  NVTB_LAUNCH_OK();
   a->stage_rows += m;
   NVTB_CUDA_OK(cudaEventRecord(a->stage_ev, st));
   a->stage_last = st;
@@ -334,7 +373,7 @@ int sortacc_stage(SortedAcc* a, const int32_t* kp, const uint8_t* mp, int64_t m,
 int sortacc_flush(SortedAcc* a, int64_t u, Counters* ctr, cudaStream_t st) {
   if (a->stage_rows == 0) return NVTB_OK;
   if (a->stage_last != st && a->stage_ev) NVTB_CUDA_OK(cudaStreamWaitEvent(st, a->stage_ev, 0));
-  int rc = sortacc_insert(a, a->stage_keys, a->stage_mask, a->stage_rows, u, ctr, st);
+  int rc = insert_rows(a, a->stage_keys, a->stage_mask, a->stage_rows, u, ctr, true, st);
   if (rc) return rc;
   a->stage_rows = 0;
   NVTB_CUDA_OK(cudaEventRecord(a->stage_ev, st));
