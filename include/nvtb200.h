@@ -425,6 +425,26 @@ int nvtb_groupstats_gather(const nvtb_groupstats_t* g,
                            void* const* out_host, const int* out_dtypes_host,
                            uint8_t* const* valid_out_host, void* stream);
 
+/* ---- row gather: the columns of Groupby, shuffle_by_keys, JoinExternal and Filter (csrc/gather.cu)
+ * Output i (i < m) reads position p = i (which 0), off[i] (1, a segment's first position) or
+ * off[i + 1] - 1 (2, its last), and row = pos ? pos[p] & row_mask : p.  A negative row (pos[p] = -1
+ * under an all-ones mask: an unmatched join row) writes 0 and a null.  Group-by callers pass the
+ * rows their ordered elements carry, row_mask = 2^row_bits - 1. */
+typedef struct {
+  const int64_t* pos;      /* may be NULL */
+  uint64_t row_mask;
+  const int64_t* off;      /* segment offsets; needed for which 1 and 2 */
+  int32_t which;
+  int32_t _pad;
+} nvtb_row_sel_t;
+/* For k < ncols (<= 16) fixed-width columns (1, 4 or 8 bytes), outs[k][i] = cols[k][row(i)], exact
+ * for every width.  valids (NULL, or per column NULL or ceil(m/8) bitmask bytes, overwritten)
+ * receive the output validity: bit i set when row(i) >= 0 and the source is valid there.  Bit k of
+ * canon_zero: column k is a float key, -0.0 is written as +0.0.  The 4/8-byte outputs 32-byte
+ * aligned, 1-byte outputs 8-byte aligned; pos has no alignment requirement. */
+int nvtb_gather_rows(const nvtb_col_t* cols, int ncols, const nvtb_row_sel_t* sel, int64_t m,
+                     void* const* outs, uint8_t* const* valids, uint32_t canon_zero, void* stream);
+
 /* ---- session group-by: Groupby operator and Dataset.shuffle_by_keys (csrc/groupby.cu, K8) ----
  * Per partition, replaces the cuDF / pandas calls of reference nvtabular/ops/groupby.py:
  * df.sort_values(sort_cols, ascending) (groupby.py:118-120), df.groupby(groupby_cols).agg(...)
@@ -478,13 +498,6 @@ int nvtb_gb_segments_write(const uint8_t* flags, const uint32_t* tile_scan, int6
 /* gid_out[p] = g for off[g] <= p < off[g + 1], p < n */
 int nvtb_gb_segment_ids(const int64_t* off, int64_t n_groups, int64_t n, uint64_t* gid_out,
                         void* stream);
-/* Gather data + validity: which 0: out[i] = col[row(i)] (i < m); 1: out[g] = col[row(off[g])];
- * 2: out[g] = col[row(off[g + 1] - 1)]; row(p) = order ? order[p] & row_mask : p.  which | 4:
- * the column is a float key, -0.0 is written as +0.0.  out_valid (may be NULL) receives
- * ceil(m/8) bitmask bytes. */
-int nvtb_gb_gather(const nvtb_col_t* col, const uint64_t* order, uint64_t row_mask,
-                   const int64_t* off, int64_t m, int which, void* out, uint8_t* out_valid,
-                   void* stream);
 /* Per segment [off[g], off[g+1]) of a column in group order, over its valid non-NaN values, in
  * fp64 and a fixed order: outs_host[7] = {count int32, sum f32, mean f32, var f32, std f32
  * (ddof 1, two passes), min, max (the column's dtype)}; NULL entries are skipped.  sum of no
@@ -578,7 +591,7 @@ int nvtb_mask_count(const uint8_t* mask, int64_t n, int64_t* tile_off, int64_t* 
 /* nvtb_mask_select (pandas boolean indexing, df[mask], then reset_index(drop=True)): rows_out
  * (n_kept int64) receives the rows whose bit is set, in ascending order, from nvtb_mask_count's
  * tile_off.  No atomics: the output is deterministic.  Moving the columns to those rows is
- * nvtb_join_gather (fixed width) and nvtb_gb_list_rows (lists). */
+ * nvtb_gather_rows (fixed width) and nvtb_gb_list_rows (lists). */
 int nvtb_mask_select(const uint8_t* mask, int64_t n, const int64_t* tile_off, int64_t* rows_out, void* stream);
 
 /* ---- external-table join: JoinExternal operator (csrc/join.cu, K9) -------------------------
@@ -615,13 +628,9 @@ int nvtb_join_probe(const nvtb_join_t* j, const nvtb_col_t* key, int64_t n, int 
  * output rows.  Outputs 32-byte aligned. */
 int nvtb_join_expand(const nvtb_join_t* j, const int64_t* ext_row_first, const int64_t* off,
                      int64_t n, int64_t n_out, int64_t* left_rows, int64_t* ext_rows, void* stream);
-/* Gather (join_external.py:148-164, the merged columns): for k < ncols (<= 16) fixed-width
- * columns, outs[k][p] = cols[k][rows[p]] for p < m, exact for every width (no fp64 round trip);
- * rows[p] = -1 writes 0 and a null.  valids (NULL, or per column NULL or ceil(m/8) bitmask bytes)
- * receive the output validity.  rows and the 4/8-byte outputs 32-byte aligned, 1-byte outputs
- * 8-byte aligned. */
-int nvtb_join_gather(const nvtb_col_t* cols, int ncols, const int64_t* rows, int64_t m,
-                     void* const* outs, uint8_t* const* valids, void* stream);
+/* The merged columns (join_external.py:148-164) are nvtb_gather_rows of the left columns at
+ * left_rows and of the ext columns at ext_rows (pos = the rows, an all-ones row_mask), and
+ * nvtb_gb_list_rows over the gathered offsets of a list column. */
 
 /* ---- cross-GPU collectives of the fit path (SURVEY.md 8e) ---------------------------------
  * nvtb_comm_t wraps an ncclComm_t: created here (rank 0 makes a unique id, the host runtime

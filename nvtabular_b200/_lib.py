@@ -9,7 +9,7 @@ import ctypes
 import os
 import threading
 from ctypes import (POINTER, Structure, c_char_p, c_double, c_int, c_int32,
-                    c_int64, c_uint8, c_uint64, c_void_p)
+                    c_int64, c_uint8, c_uint32, c_uint64, c_void_p)
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "lib", "libnvtb200.so")
@@ -29,6 +29,10 @@ class nvtb_col_t(Structure):
 class nvtb_gb_chunk_t(Structure):
     _fields_ = [("codes", c_void_p), ("valid", c_void_p), ("min", c_uint64), ("span", c_uint64),
                 ("mode", c_int32), ("lo", c_int32), ("nbits", c_int32), ("_pad", c_int32)]
+
+
+class nvtb_row_sel_t(Structure):
+    _fields_ = [("pos", c_void_p), ("row_mask", c_uint64), ("off", c_void_p), ("which", c_int32), ("_pad", c_int32)]
 
 
 class nvtb_pq_col_t(Structure):
@@ -114,8 +118,9 @@ _SIGNATURES = {
     "nvtb_gb_segments_count": (c_int, [c_void_p, c_int64, c_int, POINTER(c_void_p), c_int, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
     "nvtb_gb_segments_write": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
     "nvtb_gb_segment_ids": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
-    "nvtb_gb_gather": (c_int, [POINTER(nvtb_col_t), c_void_p, c_uint64, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
     "nvtb_gb_reduce": (c_int, [POINTER(nvtb_col_t), c_void_p, c_int64, POINTER(c_void_p), POINTER(c_void_p), c_void_p]),
+    "nvtb_gather_rows": (c_int, [POINTER(nvtb_col_t), c_int, POINTER(nvtb_row_sel_t), c_int64, POINTER(c_void_p), POINTER(c_void_p),
+                                 c_uint32, c_void_p]),
     "nvtb_gb_list_rows": (c_int, [POINTER(nvtb_col_t), c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
     "nvtb_gb_rank_stats": (c_int, [POINTER(nvtb_col_t), c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "nvtb_join_create": (c_int, [POINTER(c_void_p), c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
@@ -123,7 +128,6 @@ _SIGNATURES = {
     "nvtb_join_destroy": (c_int, [c_void_p]),
     "nvtb_join_probe": (c_int, [c_void_p, POINTER(nvtb_col_t), c_int64, c_int, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
     "nvtb_join_expand": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
-    "nvtb_join_gather": (c_int, [POINTER(nvtb_col_t), c_int, c_void_p, c_int64, POINTER(c_void_p), POINTER(c_void_p), c_void_p]),
     "nvtb_list_slice_bounds": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p]),
     "nvtb_list_slice_pad": (c_int, [POINTER(nvtb_col_t), c_void_p, c_int64, c_int64, c_int64, c_int64, c_uint64, c_void_p,
                                     c_void_p, c_void_p, c_void_p]),

@@ -304,10 +304,12 @@ inline int scan_grid(int64_t n, int ctas_per_sm) {
   return (int)g;
 }
 
-// grid for a grid-stride loop of one item per thread: at most 8 CTAs per SM
-inline int plain_grid(int64_t n) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>((n + kThreads - 1) / kThreads, (int64_t)sm_count() * 8));
+// grid for a grid-stride loop of one item per thread (per_block items per CTA): at most 8 CTAs
+// per SM
+inline int grid_for(int64_t items, int per_block) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>((items + per_block - 1) / per_block, (int64_t)sm_count() * 8));
 }
+inline int plain_grid(int64_t n) { return grid_for(n, kThreads); }
 
 // ---------------------------------------------------------------------------
 // shared-memory table hash (fold_i32.cuh, the shared-memory encode in vocab.cu): a

@@ -8,8 +8,8 @@
 // Predicates are row masks in the validity layout (LSB-first, one bit per row, padded to 32 bytes
 // like pack_validity, bits at positions >= n zero).  A mask is counted per tile of 2048 rows, the
 // tile counts are scanned by the multi-CTA scan of scan.cuh, and the kept row ids are written in
-// ascending order.  The compaction itself is the external-table join's gather (nvtb_join_gather)
-// and the sub-list copy (nvtb_gb_list_rows) at those row ids.
+// ascending order.  The compaction itself is the row gather (nvtb_gather_rows, gather.cu) and the
+// sub-list copy (nvtb_gb_list_rows) at those row ids.
 // Every mask kernel is one streaming pass in which a lane owns 8 consecutive rows, i.e. one mask
 // byte: no atomics, and the outputs are bit-identical from run to run.  Row indices are int64.
 #include "common.cuh"
@@ -29,13 +29,6 @@ struct NotnullCols {
   uint32_t vec;                         // bit q: column q may use 128-bit loads
   int32_t n;
 };
-
-inline int filt_grid(int64_t items) {
-  int64_t g = (items + kFiltThreads - 1) / kFiltThreads;
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
 
 // bytes of an n-row mask: ceil(n / 8) rounded up to whole 32-byte blocks (pack_validity's padding)
 __host__ __device__ __forceinline__ int64_t mask_bytes(int64_t n) {
@@ -258,7 +251,7 @@ int launch_compare(const nvtb_col_t* a, const nvtb_col_t* b, C s, int op, int64_
   nvtb_col_t none;
   memset(&none, 0, sizeof(none));
   const nvtb_col_t bb = b != nullptr ? *b : none;
-  mask_compare_kernel<C><<<filt_grid(mask_bytes(n)), kFiltThreads, 0, st>>>(
+  mask_compare_kernel<C><<<plain_grid(mask_bytes(n)), kFiltThreads, 0, st>>>(
       *a, vec_ok(a->data, a->dtype), bb, b != nullptr && vec_ok(b->data, b->dtype), s, op, n, out);
   NVTB_LAUNCH_OK();
   return NVTB_OK;
@@ -319,7 +312,7 @@ int nvtb_mask_notnull(const nvtb_col_t* cols, int ncols, int64_t n, uint8_t* mas
     c.dtype[q] = cols[q].dtype;
     if (vec_ok(cols[q].data, cols[q].dtype)) c.vec |= 1u << q;
   }
-  mask_notnull_kernel<<<filt_grid(mask_bytes(n)), kFiltThreads, 0, (cudaStream_t)stream>>>(c, n, mask_out);
+  mask_notnull_kernel<<<plain_grid(mask_bytes(n)), kFiltThreads, 0, (cudaStream_t)stream>>>(c, n, mask_out);
   NVTB_LAUNCH_OK();
   return NVTB_OK;
 }
@@ -331,7 +324,7 @@ int nvtb_mask_logic(const uint8_t* a, const uint8_t* b, int64_t n, int op, uint8
   NVTB_REQUIRE(a != nullptr && out != nullptr && (op == NVTB_MASK_NOT || b != nullptr), "NULL mask");
   const auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
   NVTB_REQUIRE(al16(a) && al16(out) && (b == nullptr || al16(b)), "masks must be 16-byte aligned");
-  mask_logic_kernel<<<filt_grid(mask_bytes(n) / 16), kFiltThreads, 0, (cudaStream_t)stream>>>(
+  mask_logic_kernel<<<plain_grid(mask_bytes(n) / 16), kFiltThreads, 0, (cudaStream_t)stream>>>(
       reinterpret_cast<const uint4*>(a), op == NVTB_MASK_NOT ? nullptr : reinterpret_cast<const uint4*>(b), n, op,
       reinterpret_cast<uint4*>(out));
   NVTB_LAUNCH_OK();
@@ -346,7 +339,7 @@ int nvtb_mask_count(const uint8_t* mask, int64_t n, int64_t* tile_off, int64_t* 
   NVTB_REQUIRE(tile_off != nullptr && is_aligned32(tile_off), "tile_off must be non-NULL and 32-byte aligned");
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t ntiles = (n + kMaskTile - 1) / kMaskTile;
-  mask_tile_count_kernel<<<filt_grid(ntiles * 32), kFiltThreads, 0, st>>>(mask, n, ntiles, tile_off);
+  mask_tile_count_kernel<<<plain_grid(ntiles * 32), kFiltThreads, 0, st>>>(mask, n, ntiles, tile_off);
   NVTB_LAUNCH_OK();
   return excl_scan_i64(tile_off, ntiles, n_kept_host, st);
 }

@@ -14,7 +14,7 @@
 //   2. order rows    LSD rounds of the radix primitive (radix.cuh, rx_sort_bits) over elements
 //                    (packed fields << r) | row; every round rewrites the high bits in place
 //   3. segments      boundary flags of the sorted rows + a tile scan -> int64 group offsets
-//   4. gather        one gather per value column into group order (the `list` leaves)
+//   4. gather        the value columns into group order (the `list` leaves; gather.cu)
 //   5. reduce        count / sum / mean / var / std / min / max per segment in fp64, in a
 //                    fixed order (warp per segment; long segments one CTA each)
 //   6. rank stats    median / nunique over rows ordered by (group, value) with stage 2
@@ -51,10 +51,6 @@ struct KeyCodes {
   const uint64_t* codes[kMaxKeys];
   int n;
 };
-
-__device__ __forceinline__ bool bit_at(const uint8_t* __restrict__ m, int64_t i) {
-  return m == nullptr || ((__ldg(m + (i >> 3)) >> (i & 7)) & 1u);
-}
 
 // ---------------------------------------------------------------------------------------
 // 1. order codes
@@ -145,7 +141,7 @@ codes_kernel(const T* __restrict__ data, const uint8_t* __restrict__ mask, int64
 // 2. one LSD round: rewrite the high bits of every element from its row's codes
 // ---------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t field_value(const Chunk& c, uint64_t row) {
-  const bool ok = bit_at(c.valid, (int64_t)row);
+  const bool ok = valid1(c.valid, (int64_t)row);
   switch (c.mode) {
     case 0: return c.codes[row] - c.min;
     case 1: return ok ? c.codes[row] - c.min : c.span + 1;
@@ -218,7 +214,7 @@ seg_flags_kernel(const uint64_t* __restrict__ order, int64_t n, int row_bits, Ke
     for (int k = 0; k < 8 && p0 + k < n; ++k) {
       const int64_t p = p0 + k;
       const uint64_t row = order[p] & row_mask;
-      if (bit_at(key_valid, (int64_t)row)) {
+      if (valid1(key_valid, (int64_t)row)) {
         kv |= 1u << k;
         bool differs = p == 0;
         for (int j = 0; j < keys.n && !differs; ++j) differs = keys.codes[j][row] != keys.codes[j][prev];
@@ -282,36 +278,6 @@ segment_ids_kernel(const int64_t* __restrict__ off, int64_t n_groups, int64_t n,
 }
 
 // ---------------------------------------------------------------------------------------
-// 4. gathers
-// ---------------------------------------------------------------------------------------
-// which & 3 = 0: out[i] = src[row(i)], i < m;  1: out[g] = src[row(off[g])];  2: out[g] = src[row(off[g+1]-1)]
-// row(p) = order ? order[p] & row_mask : p.  Every lane writes 8 consecutive outputs (one
-// validity byte).
-template <typename T>
-__global__ void __launch_bounds__(kGbThreads)
-gather_kernel(const T* __restrict__ src, const uint8_t* __restrict__ src_valid, const uint64_t* __restrict__ order,
-              uint64_t row_mask, const int64_t* __restrict__ off, int64_t m, int which, T* __restrict__ out,
-              uint8_t* __restrict__ out_valid) {
-  const int64_t ngroups = (m + 7) / 8;
-  for (int64_t gi = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; gi < ngroups; gi += (int64_t)gridDim.x * blockDim.x) {
-    unsigned vb = 0;
-    for (int k = 0; k < 8; ++k) {
-      const int64_t i = gi * 8 + k;
-      if (i >= m) break;
-      const int w = which & 3;
-      const int64_t p = w == 0 ? i : (w == 1 ? off[i] : off[i + 1] - 1);
-      const int64_t row = order != nullptr ? (int64_t)(order[p] & row_mask) : p;
-      T x = src[row];
-      // which | 4: a float key, -0.0 becomes +0.0 (the bit pattern of the sign alone)
-      if ((which & 4) && sizeof(T) >= 4 && x == ((T)1 << (8 * sizeof(T) - 1))) x = 0;
-      out[i] = x;
-      if (bit_at(src_valid, row)) vb |= 1u << k;
-    }
-    if (out_valid != nullptr) out_valid[gi] = (uint8_t)vb;
-  }
-}
-
-// ---------------------------------------------------------------------------------------
 // 5. segmented reductions
 // ---------------------------------------------------------------------------------------
 struct ReduceOut {
@@ -333,7 +299,7 @@ struct Acc {
 
 template <typename T>
 __device__ __forceinline__ bool load_value(const T* __restrict__ d, const uint8_t* __restrict__ v, int64_t p, T& x) {
-  if (!bit_at(v, p)) return false;
+  if (!valid1(v, p)) return false;
   x = d[p];
   if constexpr (std::is_floating_point<T>::value) return !isnan(x);
   return true;
@@ -505,7 +471,7 @@ rank_stats_kernel(const T* __restrict__ d, const uint64_t* __restrict__ codes, c
     int64_t lo = s, hi = e;                   // first invalid position in [s, e]
     while (lo < hi) {
       const int64_t mid = (lo + hi) >> 1;
-      if (bit_at(cvalid, (int64_t)(order[mid] & row_mask))) lo = mid + 1; else hi = mid;
+      if (valid1(cvalid, (int64_t)(order[mid] & row_mask))) lo = mid + 1; else hi = mid;
     }
     const int64_t cnt = lo - s;
     if (nunique != nullptr) {
@@ -570,7 +536,7 @@ list_copy_kernel(const T* __restrict__ src, const uint8_t* __restrict__ src_vali
       const int64_t g = last_at_or_below(off, g0, g1 + 1, p);
       const int64_t s = __ldg(lo + g) + (p - __ldg(off + g));
       v[k] = src[s];
-      if (p0 + k <= pe && bit_at(src_valid, s)) vb |= 1u << k;
+      if (p0 + k <= pe && valid1(src_valid, s)) vb |= 1u << k;
     }
     if (aligned && p0 + 8 <= total) {
       st_rows8<T>(out + p0, v);
@@ -580,13 +546,6 @@ list_copy_kernel(const T* __restrict__ src, const uint8_t* __restrict__ src_vali
     }
     if (out_valid != nullptr) out_valid[p0 >> 3] = (uint8_t)vb;
   }
-}
-
-inline int grid_for(int64_t items, int per_block) {
-  int64_t g = (items + per_block - 1) / per_block;
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
 }
 
 }  // namespace
@@ -716,24 +675,6 @@ int nvtb_gb_segment_ids(const int64_t* off, int64_t n_groups, int64_t n, uint64_
   if (n == 0) return NVTB_OK;
   NVTB_REQUIRE(off && gid_out && n_groups > 0, "NULL buffers");
   segment_ids_kernel<<<grid_for(n, kGbThreads), kGbThreads, 0, (cudaStream_t)stream>>>(off, n_groups, n, gid_out);
-  NVTB_LAUNCH_OK();
-  return NVTB_OK;
-}
-
-int nvtb_gb_gather(const nvtb_col_t* col, const uint64_t* order, uint64_t row_mask, const int64_t* off, int64_t m,
-                   int which, void* out, uint8_t* out_valid, void* stream) {
-  NVTB_REQUIRE(col != nullptr && m >= 0 && (which & 3) <= 2 && (which & ~7) == 0, "bad arguments");
-  NVTB_REQUIRE((which & 3) == 0 || off != nullptr, "segment ends need offsets");
-  if (m == 0) return NVTB_OK;
-  NVTB_REQUIRE(col->data && out, "NULL data / out");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int grid = grid_for((m + 7) / 8, kGbThreads);
-  switch (dtype_size(col->dtype)) {
-    case 1: gather_kernel<uint8_t><<<grid, kGbThreads, 0, st>>>((const uint8_t*)col->data, col->validity, order, row_mask, off, m, which, (uint8_t*)out, out_valid); break;
-    case 4: gather_kernel<uint32_t><<<grid, kGbThreads, 0, st>>>((const uint32_t*)col->data, col->validity, order, row_mask, off, m, which, (uint32_t*)out, out_valid); break;
-    case 8: gather_kernel<uint64_t><<<grid, kGbThreads, 0, st>>>((const uint64_t*)col->data, col->validity, order, row_mask, off, m, which, (uint64_t*)out, out_valid); break;
-    default: set_error("nvtb_gb_gather: unsupported dtype %d", (int)col->dtype); return NVTB_EINVAL;
-  }
   NVTB_LAUNCH_OK();
   return NVTB_OK;
 }

@@ -13,7 +13,7 @@
 //           scanned into int64 output offsets
 //   expand  (duplicated keys / inner joins) per output row, its left row and ext row; balanced
 //           over OUTPUT rows, so one key with 10^6 matches does not serialise on one thread
-//   gather  up to 16 fixed-width columns at int64 rows per launch, -1 = null
+// The columns are then gathered at those rows by gather.cu (-1 = null).
 // Int32 holds every count and group id: the ext table has fewer than 2^31 rows.
 #include <cstring>
 #include <new>
@@ -25,23 +25,6 @@ namespace nvtb {
 namespace {
 
 constexpr int kJoinThreads = 256;
-constexpr int kMaxJoinCols = 16;
-
-struct JoinCols {
-  const void* src[kMaxJoinCols];
-  const uint8_t* src_valid[kMaxJoinCols];
-  void* out[kMaxJoinCols];
-  uint8_t* out_valid[kMaxJoinCols];
-  int32_t size[kMaxJoinCols];
-  int32_t ncols;
-};
-
-inline int join_grid(int64_t items) {
-  int64_t g = (items + kJoinThreads - 1) / kJoinThreads;
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
 
 // ---------------------------------------------------------------------------------------
 // build: a wide table key -> run index g (keys are distinct: they come out of K8 segments)
@@ -161,53 +144,6 @@ join_expand_kernel(const int64_t* __restrict__ first, const int64_t* __restrict_
   }
 }
 
-// ---------------------------------------------------------------------------------------
-// gather: every lane owns 8 consecutive output rows, i.e. one validity byte of every output, so
-// the bitmasks are written without atomics.  Row -1 gives a null (data 0).
-// ---------------------------------------------------------------------------------------
-template <typename T>
-__device__ __forceinline__ void gather8(const JoinCols& c, int j, const int64_t (&r)[8], int64_t i, int64_t m) {
-  const T* __restrict__ src = static_cast<const T*>(c.src[j]);
-  const uint8_t* __restrict__ sv = c.src_valid[j];
-  T v[8];
-  unsigned vb = 0;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const bool ok = i + k < m && r[k] >= 0;
-    v[k] = ok ? src[r[k]] : (T)0;
-    if (ok && valid1(sv, r[k])) vb |= 1u << k;
-  }
-  T* out = static_cast<T*>(c.out[j]);
-  if (i + 8 <= m) {
-    st_rows8<T>(out + i, v);
-  } else {
-#pragma unroll
-    for (int k = 0; k < 8; ++k) if (i + k < m) out[i + k] = v[k];
-  }
-  if (c.out_valid[j] != nullptr) c.out_valid[j][i >> 3] = (uint8_t)vb;
-}
-
-__global__ void __launch_bounds__(kJoinThreads)
-join_gather_kernel(const int64_t* __restrict__ rows, int64_t m, JoinCols c) {
-  const int64_t nchunks = (m + 7) / 8;
-  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < nchunks; g += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t i = g * 8;
-    int64_t r[8];
-    load8_i64(rows, i, m, r);
-    if (i + 8 > m) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) if (i + k >= m) r[k] = -1;
-    }
-    for (int j = 0; j < c.ncols; ++j) {
-      switch (c.size[j]) {
-        case 1: gather8<uint8_t>(c, j, r, i, m); break;
-        case 4: gather8<uint32_t>(c, j, r, i, m); break;
-        default: gather8<int64_t>(c, j, r, i, m); break;
-      }
-    }
-  }
-}
-
 }  // namespace
 }  // namespace nvtb
 
@@ -253,9 +189,9 @@ int nvtb_join_create(nvtb_join_t** out, const int64_t* distinct_keys, int64_t n_
     if (cudaMemcpyAsync(scal, h, sizeof(h), cudaMemcpyHostToDevice, st) != cudaSuccess) break;
     if (n_groups > 0 && cudaMemcpyAsync(j->off, off, sizeof(int64_t) * (n_groups + 1), cudaMemcpyDeviceToDevice, st) != cudaSuccess) break;
     if (n_ext > 0 && cudaMemcpyAsync(j->rows, ordered_rows, sizeof(int64_t) * n_ext, cudaMemcpyDeviceToDevice, st) != cudaSuccess) break;
-    join_table_init_kernel<<<join_grid(j->t.capacity), kJoinThreads, 0, st>>>(j->t.slots, j->t.capacity);
+    join_table_init_kernel<<<plain_grid(j->t.capacity), kJoinThreads, 0, st>>>(j->t.slots, j->t.capacity);
     if (n_groups > 0)
-      join_table_build_kernel<<<join_grid(n_groups), kJoinThreads, 0, st>>>(distinct_keys, off, n_groups, j->t.slots,
+      join_table_build_kernel<<<plain_grid(n_groups), kJoinThreads, 0, st>>>(distinct_keys, off, n_groups, j->t.slots,
                                                                              j->t.capacity, scal);
     if (cudaGetLastError() != cudaSuccess) break;
     if (cudaMemcpyAsync(h, scal, sizeof(h), cudaMemcpyDeviceToHost, st) != cudaSuccess) break;
@@ -303,7 +239,7 @@ int nvtb_join_probe(const nvtb_join_t* j, const nvtb_col_t* key, int64_t n, int 
   if (off_out == nullptr && n == 0) return NVTB_OK;
   if (n > 0) {
     NVTB_REQUIRE(key->data != nullptr && ext_row_out != nullptr, "NULL key data / ext_row_out");
-    const int grid = join_grid(n);
+    const int grid = plain_grid(n);
     const int left = how == 0;
     if (key->dtype == NVTB_I32)
       join_probe_kernel<int32_t><<<grid, kJoinThreads, 0, st>>>((const int32_t*)key->data, key->validity, n, j->t, j->off,
@@ -323,34 +259,8 @@ int nvtb_join_expand(const nvtb_join_t* j, const int64_t* ext_row_first, const i
   if (n_out == 0) return NVTB_OK;
   NVTB_REQUIRE(n > 0 && ext_row_first && off && left_rows && ext_rows, "NULL buffers");
   NVTB_REQUIRE(is_aligned32(left_rows) && is_aligned32(ext_rows), "outputs must be 32-byte aligned");
-  join_expand_kernel<<<join_grid((n_out + 7) / 8), kJoinThreads, 0, (cudaStream_t)stream>>>(
+  join_expand_kernel<<<plain_grid((n_out + 7) / 8), kJoinThreads, 0, (cudaStream_t)stream>>>(
       ext_row_first, off, n, n_out, j->rows, left_rows, ext_rows);
-  NVTB_LAUNCH_OK();
-  return NVTB_OK;
-}
-
-int nvtb_join_gather(const nvtb_col_t* cols, int ncols, const int64_t* rows, int64_t m, void* const* outs,
-                     uint8_t* const* valids, void* stream) {
-  NVTB_REQUIRE(cols != nullptr && outs != nullptr && m >= 0, "NULL argument or m < 0");
-  NVTB_REQUIRE(ncols >= 1 && ncols <= kMaxJoinCols, "ncols must be in [1, 16]");
-  if (m == 0) return NVTB_OK;
-  NVTB_REQUIRE(rows != nullptr && is_aligned32(rows), "rows must be non-NULL and 32-byte aligned");
-  JoinCols c;
-  memset(&c, 0, sizeof(c));
-  c.ncols = ncols;
-  for (int k = 0; k < ncols; ++k) {
-    const int sz = (int)dtype_size(cols[k].dtype);
-    NVTB_REQUIRE(sz == 1 || sz == 4 || sz == 8, "unsupported column dtype");
-    NVTB_REQUIRE(cols[k].data != nullptr && outs[k] != nullptr, "NULL column data / output");
-    NVTB_REQUIRE(sz == 1 ? (reinterpret_cast<uintptr_t>(outs[k]) & 7u) == 0 : is_aligned32(outs[k]),
-                 "outputs must be 32-byte aligned (uint8: 8-byte)");
-    c.src[k] = cols[k].data;
-    c.src_valid[k] = cols[k].validity;
-    c.out[k] = outs[k];
-    c.out_valid[k] = valids != nullptr ? valids[k] : nullptr;
-    c.size[k] = sz;
-  }
-  join_gather_kernel<<<join_grid((m + 7) / 8), kJoinThreads, 0, (cudaStream_t)stream>>>(rows, m, c);
   NVTB_LAUNCH_OK();
   return NVTB_OK;
 }

@@ -38,13 +38,6 @@ struct LagCols {
   int32_t ncols;
 };
 
-inline int sess_grid(int64_t items) {
-  int64_t g = (items + kSessThreads - 1) / kSessThreads;
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
-
 // ---------------------------------------------------------------------------------------
 // ListSlice
 // ---------------------------------------------------------------------------------------
@@ -249,7 +242,7 @@ int nvtb_list_slice_bounds(const int64_t* offsets, int64_t n, int64_t start, int
   NVTB_REQUIRE(n >= 0, "n < 0");
   if (n == 0) return NVTB_OK;
   NVTB_REQUIRE(offsets && lo_out && hi_out, "NULL offsets / outputs");
-  list_slice_bounds_kernel<<<sess_grid(n), kSessThreads, 0, (cudaStream_t)stream>>>(offsets, n, start, end, lo_out,
+  list_slice_bounds_kernel<<<plain_grid(n), kSessThreads, 0, (cudaStream_t)stream>>>(offsets, n, start, end, lo_out,
                                                                                     hi_out);
   NVTB_LAUNCH_OK();
   return NVTB_OK;
@@ -266,7 +259,7 @@ int nvtb_list_slice_pad(const nvtb_col_t* leaves, const int64_t* offsets, int64_
   NVTB_REQUIRE(sz == 1 ? (reinterpret_cast<uintptr_t>(out) & 7u) == 0 : is_aligned32(out),
                "out must be 32-byte aligned (1-byte leaves: 8-byte)");
   cudaStream_t st = (cudaStream_t)stream;
-  const int grid = sess_grid((n * L + 7) / 8 > n + 1 ? (n * L + 7) / 8 : n + 1);
+  const int grid = plain_grid((n * L + 7) / 8 > n + 1 ? (n * L + 7) / 8 : n + 1);
   switch (sz) {
 #define NVTB_PAD_LAUNCH(T)                                                                                  \
   {                                                                                                         \
@@ -299,7 +292,7 @@ int nvtb_lag_same_key(const nvtb_col_t* keys, int n_keys, int64_t n, int64_t shi
     k.valid[q] = keys[q].validity;
     k.dtype[q] = keys[q].dtype;
   }
-  lag_same_key_kernel<<<sess_grid((n + 7) / 8), kSessThreads, 0, (cudaStream_t)stream>>>(k, n, clamp_shift(shift, n),
+  lag_same_key_kernel<<<plain_grid((n + 7) / 8), kSessThreads, 0, (cudaStream_t)stream>>>(k, n, clamp_shift(shift, n),
                                                                                          same_out);
   NVTB_LAUNCH_OK();
   return NVTB_OK;
@@ -326,7 +319,7 @@ int nvtb_difference_lag(const nvtb_col_t* cols, int ncols, int64_t n, int64_t sh
     c.out_valid[q] = out_valids[q];
     c.dtype[q] = dt;
   }
-  difference_lag_kernel<<<sess_grid((n + 7) / 8), kSessThreads, 0, (cudaStream_t)stream>>>(c, n, clamp_shift(shift, n),
+  difference_lag_kernel<<<plain_grid((n + 7) / 8), kSessThreads, 0, (cudaStream_t)stream>>>(c, n, clamp_shift(shift, n),
                                                                                            same);
   NVTB_LAUNCH_OK();
   return NVTB_OK;

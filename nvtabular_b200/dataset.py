@@ -374,13 +374,11 @@ class Dataset:
             lo, hi = (int(x) for x in stats[:2].cpu().numpy().view(np.uint64))
             order, r = _order_rows([(dcodes, None, lo, hi - lo, 0, (hi - lo).bit_length())], n, dev)
             off, g, _ = engine.gb_segments(order, r, [dcodes], None)
-            seg_dest = engine.gb_gather(Column(dest), order, r, g, 1, off).data.cpu().tolist()
+            seg_dest = engine.take_rows({"dest": Column(dest)}, engine.order_sel(order, r, 1, off), g)["dest"]
             bounds = off.cpu().tolist()
-            for j, d in enumerate(seg_dest):
-                piece_order = order[bounds[j]: bounds[j + 1]]
-                pieces[d].append(DeviceFrame({
-                    name: engine.gb_gather(c, piece_order, r, bounds[j + 1] - bounds[j], 0)
-                    for name, c in part.items()}))
+            for j, d in enumerate(seg_dest.data.cpu().tolist()):
+                piece = engine.order_sel(order[bounds[j]: bounds[j + 1]], r)
+                pieces[d].append(DeviceFrame(engine.take_rows(dict(part.items()), piece, bounds[j + 1] - bounds[j])))
         if template is None:
             return Dataset([DeviceFrame()])
         dicts = {}

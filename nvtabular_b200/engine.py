@@ -8,7 +8,7 @@ buffers and to read back O(#columns) scalars.
 import ctypes
 import os
 from ctypes import byref, c_int, c_int64, c_void_p
-from typing import List, Optional, Sequence
+from typing import List, NamedTuple, Optional, Sequence
 
 import numpy as np
 import torch
@@ -242,8 +242,7 @@ def pack_keys2(a: Column, b: Column) -> Column:
     n = _check_same_len([a, b])
     keys = torch.empty(n, dtype=torch.int64, device=a.data.device)
     need_mask = a.validity is not None and b.validity is not None
-    nbytes = (((n + 7) // 8 + 31) // 32) * 32
-    mask = torch.zeros(nbytes, dtype=torch.uint8, device=a.data.device) if need_mask else None
+    mask = _bitmask(n, a.data.device) if need_mask else None
     _lib.check(lib.nvtb_pack_keys2(_descs([a]), _descs([b]), n, _ptr(keys), _ptr(mask), _lib.stream_ptr()))
     _count()
     return Column(keys, mask)
@@ -649,8 +648,7 @@ class GroupStats:
         dev = key.data.device
         codes = [dtype_code(d) for d in out_dtypes]
         outs = [torch.empty(n, dtype=_CODE2TORCH[c], device=dev) for c in codes]
-        nbytes = (((n + 7) // 8 + 31) // 32) * 32          # pack_validity's padding (>= ceil(n/32) words)
-        valid = [torch.zeros(nbytes, dtype=torch.uint8, device=dev) if j < len(masked) and masked[j] else None
+        valid = [_bitmask(n, dev) if j < len(masked) and masked[j] else None
                  for j in range(len(cols))]
         for s in range(0, len(cols), self.MAX_COLS):
             e = s + self.MAX_COLS
@@ -663,10 +661,76 @@ class GroupStats:
         return [Column(o, v) for o, v in zip(outs, valid)]
 
 
+# ------------------------------------------------------------- row gather (csrc/gather.cu)
+GATHER_MAX_COLS = 16   # columns of one nvtb_gather_rows launch (kMaxGatherCols, csrc/gather.cu)
+ALL_ROWS = (1 << 64) - 1
+
+
+class RowSel(NamedTuple):
+    """The rows a gather reads (nvtb_row_sel_t): output i reads position p = i, off[i] or off[i + 1] - 1
+    (which 0, 1, 2) at row pos[p] & row_mask, or p without pos; a negative row (-1: ALL_ROWS) is null."""
+    pos: Optional[torch.Tensor] = None
+    row_mask: int = ALL_ROWS
+    off: Optional[torch.Tensor] = None
+    which: int = 0
+
+
+def order_sel(order: torch.Tensor, row_bits: int, which: int = 0, off: Optional[torch.Tensor] = None) -> RowSel:
+    """the rows of ordered group-by elements (packed fields << row_bits | row, gb_order_rows)"""
+    return RowSel(order, (1 << row_bits) - 1, off, which)
+
+
+def gather(cols: Sequence[Column], sel, m: int, masked: bool = False, canon_zero: Sequence[bool] = ()) -> List[Column]:
+    """m rows of flat columns at `sel` (a RowSel, or int64 rows with -1 = null) -> Columns with the
+    sources' dtype, dictionary and bool flag (nvtb_gather_rows, GATHER_MAX_COLS columns per
+    launch).  An output gets a validity bitmask when its source has one or `masked`; with
+    canon_zero[k], column k is a float key and -0.0 is written as +0.0."""
+    if not cols:
+        return []
+    lib = _lib.load()
+    sel = sel if isinstance(sel, RowSel) else RowSel(sel)
+    dev = cols[0].data.device
+    # an empty source (an empty ext table) is only ever read at row -1: give the kernel one row
+    cols = [c if c.data.numel() else Column(torch.zeros(1, dtype=c.data.dtype, device=dev), None, None,
+                                            c.dictionary, None, c.is_bool) for c in cols]
+    outs = [torch.empty(max(m, 1), dtype=c.data.dtype, device=dev) for c in cols]
+    valids = [_bitmask(m, dev) if (masked or c.validity is not None) else None for c in cols]
+    canon = sum(1 << k for k, z in enumerate(canon_zero) if z)
+    csel = _lib.nvtb_row_sel_t(_ptr(sel.pos), sel.row_mask, _ptr(sel.off), sel.which, 0)
+    index_bytes = m * 8.0 * ((sel.pos is not None) + (sel.which != 0))
+    for s in range(0, len(cols), GATHER_MAX_COLS):
+        e = s + GATHER_MAX_COLS
+        nbytes = index_bytes + sum(m * (c.data.element_size() * 2.0 + (0.125 if v is not None else 0.0))
+                                   for c, v in zip(cols[s:e], valids[s:e]))
+        with _timed("gather", nbytes):
+            _lib.check(lib.nvtb_gather_rows(_descs(cols[s:e]), len(cols[s:e]), byref(csel), m,
+                                            _lib.ptr_array([o.data_ptr() for o in outs[s:e]]),
+                                            _lib.ptr_array([v.data_ptr() if v is not None else None
+                                                            for v in valids[s:e]]),
+                                            (canon >> s) & ((1 << GATHER_MAX_COLS) - 1), _lib.stream_ptr()))
+        _count()
+    return [Column(o[:m], v, None, c.dictionary, None, c.is_bool) for o, v, c in zip(outs, valids, cols)]
+
+
+def take_rows(cols, sel, m: Optional[int] = None, masked: bool = False):
+    """{name: Column} at the m rows of `sel` (int64 rows, -1 = null, m = their count; or a RowSel):
+    fixed-width columns through gather, list columns through nvtb_gb_list_rows over their offsets,
+    gathered in one more call.  With `masked`, row -1 is null (an empty list for a list column)."""
+    m = sel.numel() if m is None else m
+    flat = [n for n, c in cols.items() if not c.is_list]
+    lists = [n for n, c in cols.items() if c.is_list]
+    res = dict(zip(flat, gather([cols[n] for n in flat], sel, m, masked)))
+    if lists:
+        bounds = gather([Column(b) for n in lists for b in (cols[n].offsets[:-1], cols[n].offsets[1:])], sel, m)
+        for k, n in enumerate(lists):
+            res[n] = gb_list_rows(cols[n].leaves(), bounds[2 * k].data, bounds[2 * k + 1].data)
+    return {n: res[n] for n in cols}
+
+
 # ------------------------------------------------------------- session group-by (K8, csrc/groupby.cu)
 def _bitmask(n: int, device) -> torch.Tensor:
     """a zeroed validity bitmask of n bits in pack_validity's padding (whole 32-byte blocks)"""
-    return torch.zeros((((n + 7) // 8 + 31) // 32) * 32, dtype=torch.uint8, device=device)
+    return torch.zeros(mask_nbytes(n), dtype=torch.uint8, device=device)
 
 
 def gb_order_codes(col: Column, stats: torch.Tensor, key_valid: Optional[torch.Tensor] = None, and_key_valid=False):
@@ -728,21 +792,6 @@ def gb_segment_ids(off: torch.Tensor, n_groups: int, n: int) -> torch.Tensor:
     _lib.check(lib.nvtb_gb_segment_ids(_ptr(off), n_groups, n, _ptr(gid), _lib.stream_ptr()))
     _count()
     return gid
-
-
-def gb_gather(col: Column, order: Optional[torch.Tensor], row_bits: int, m: int, which: int = 0,
-              off: Optional[torch.Tensor] = None) -> Column:
-    """data + validity of `col` at row(i) (which 0), at the first (1) or last (2) position of every
-    segment; row(p) = order[p] & (2^row_bits - 1), or p without an order (nvtb_gb_gather)"""
-    lib = _lib.load()
-    dev = col.data.device
-    out = torch.empty(m, dtype=col.data.dtype, device=dev)
-    valid = _bitmask(m, dev) if col.validity is not None else None
-    with _timed("groupby_gather", m * (col.data.element_size() * 2 + (8 if order is not None else 0))):
-        _lib.check(lib.nvtb_gb_gather(_descs([col]), _ptr(order), (1 << row_bits) - 1, _ptr(off), m, which,
-                                      _ptr(out), _ptr(valid), _lib.stream_ptr()))
-    _count()
-    return Column(out, valid, None, col.dictionary, None, col.is_bool)
 
 
 def gb_reduce(col: Column, off: torch.Tensor, n_groups: int, aggs: Sequence[str]):
@@ -931,46 +980,6 @@ class JoinTable:
                                                  _ptr(ext), _lib.stream_ptr()))
         _count()
         return left[:n_out], ext[:n_out]
-
-
-JOIN_GATHER_MAX_COLS = 16   # columns of one nvtb_join_gather launch (kMaxJoinCols, csrc/join.cu)
-
-
-def join_gather(cols: Sequence[Column], rows: torch.Tensor, masked: Sequence[bool]) -> List[Column]:
-    """flat columns at int64 `rows` (-1 = null) -> Columns with the sources' dtype, dictionary and
-    bool flag; output k gets a validity bitmask when masked[k] or its source has one
-    (nvtb_join_gather)"""
-    lib = _lib.load()
-    m = rows.numel()
-    dev = rows.device
-    # an empty source (an empty ext table) is only ever read at row -1: give the kernel one row
-    cols = [c if c.data.numel() else Column(torch.zeros(1, dtype=c.data.dtype, device=dev), None, None,
-                                            c.dictionary, None, c.is_bool) for c in cols]
-    outs = [torch.empty(max(m, 1), dtype=c.data.dtype, device=dev) for c in cols]
-    valids = [_bitmask(m, dev) if (mk or c.validity is not None) else None for c, mk in zip(cols, masked)]
-    for s in range(0, len(cols), JOIN_GATHER_MAX_COLS):
-        e = s + JOIN_GATHER_MAX_COLS
-        nbytes = m * 8.0 + sum(m * (c.data.element_size() + 0.125) for c in cols[s:e])
-        with _timed("join_gather", nbytes):
-            _lib.check(lib.nvtb_join_gather(_descs(cols[s:e]), len(cols[s:e]), _ptr(rows), m,
-                                            _lib.ptr_array([o.data_ptr() for o in outs[s:e]]),
-                                            _lib.ptr_array([v.data_ptr() if v is not None else None
-                                                            for v in valids[s:e]]), _lib.stream_ptr()))
-        _count()
-    return [Column(o[:m], v, None, c.dictionary, None, c.is_bool) for o, v, c in zip(outs, valids, cols)]
-
-
-def take_rows(cols, rows: torch.Tensor, masked: bool = False):
-    """{name: Column} at int64 `rows`, in the same order; a fixed-width column through
-    nvtb_join_gather, a list column through nvtb_gb_list_rows over its gathered offsets.  With
-    `masked`, row -1 is null (an empty list for a list column)."""
-    flat = [n for n, c in cols.items() if not c.is_list]
-    res = dict(zip(flat, join_gather([cols[n] for n in flat], rows, [masked] * len(flat)))) if flat else {}
-    for n, c in cols.items():
-        if c.is_list:
-            lo, hi = join_gather([Column(c.offsets[:-1]), Column(c.offsets[1:])], rows, [False, False])
-            res[n] = gb_list_rows(c.leaves(), lo.data, hi.data)
-    return {n: res[n] for n in cols}
 
 
 # ------------------------------------------------------------- row selection (K11, csrc/filter.cu)

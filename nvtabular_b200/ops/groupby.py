@@ -202,26 +202,24 @@ class Groupby(Operator):
         if g == 0:
             return self._empty(outputs, cols)
 
-        # 4-6. values
-        out = DeviceFrame()
-        bufs: Dict[str, Column] = {}
+        # 4-6. values: the keys at every group's first row, the value columns in group order
+        key_out = {name: cols[src] for name, (src, agg) in outputs.items() if agg is None}
+        out = dict(zip(key_out, engine.gather(list(key_out.values()), engine.order_sel(order, r, 1, off), g,
+                                              canon_zero=[c.data.dtype.is_floating_point for c in key_out.values()])))
+        srcs = list(dict.fromkeys(s for s, a in outputs.values() if a is not None and not cols[s].is_list))
+        bufs = dict(zip(srcs, engine.gather([cols[s] for s in srcs], engine.order_sel(order, r), kept)))
+        for end in (1, 2):
+            ends = {name: src for name, (src, agg) in outputs.items()
+                    if agg in ("first", "last") and self._end(agg) == end}
+            flat = {name: bufs[src] for name, src in ends.items() if not cols[src].is_list}
+            lists = {name: cols[src] for name, src in ends.items() if cols[src].is_list}
+            out.update(engine.take_rows(flat, engine.RowSel(off=off, which=end), g))
+            out.update(engine.take_rows(lists, engine.order_sel(order, r, end, off), g))
         rank_cols = {}
         for name, (src, agg) in outputs.items():
-            c = cols[src]
-            if agg is None:
-                which = 1 | (4 if c.data.dtype.is_floating_point else 0)
-                out[name] = engine.gb_gather(c, order, r, g, which, off)
-                continue
-            if c.is_list:
-                out[name] = _first_last_of_lists(c, order, r, off, g, self._end(agg))
-                continue
-            if src not in bufs:
-                bufs[src] = engine.gb_gather(c, order, r, kept, 0)
-            buf = bufs[src]
             if agg == "list":
+                buf = bufs[src]
                 out[name] = Column(buf.data, buf.validity, off, buf.dictionary, None, buf.is_bool)
-            elif agg in ("first", "last"):
-                out[name] = engine.gb_gather(buf, None, 0, g, self._end(agg), off)
             elif agg in ("median", "nunique"):
                 rank_cols.setdefault(src, set()).add(agg)
         reduced = {}
@@ -307,9 +305,3 @@ def _rank_stats(bufs, wanted, off, g, kept, dev):
             res[(s, "nunique")] = Column(nun)
     return res
 
-
-def _first_last_of_lists(c: Column, order, r, off, g, which) -> Column:
-    """`first` / `last` of a list column: the sub-list of the segment's first / last row"""
-    lo = engine.gb_gather(Column(c.offsets[:-1], None), order, r, g, which, off).data
-    hi = engine.gb_gather(Column(c.offsets[1:], None), order, r, g, which, off).data
-    return engine.gb_list_rows(Column(c.data, c.validity, None, c.dictionary, None, c.is_bool), lo, hi)

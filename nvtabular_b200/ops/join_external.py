@@ -187,7 +187,7 @@ class _Table:
                                     torch.arange(n, dtype=torch.int64, device=dev), 0, n)
         order, r = _order_rows(fields, n, dev)
         off, g, kept = engine.gb_segments(order, r, [codes], valid)
-        distinct = engine.gb_gather(Column(key.data, None), order, r, g, 1, off).data
+        distinct = engine.take_rows({"key": Column(key.data)}, engine.order_sel(order, r, 1, off), g)["key"].data
         rows = order & ((1 << r) - 1)
         return engine.JoinTable(distinct, off, rows, kept, n)
 

@@ -14,7 +14,7 @@ item_id int32, ts int64, price float32 uniform in [0, 100)):
                  measures the compaction of the list column
 Every workload reports the whole operator call and its families, each timed alone with CUDA events
 (median of `steps` after `warmup`): mask (nvtb_mask_compare / nvtb_mask_notnull), count
-(nvtb_mask_count, with its host read), select (nvtb_mask_select), gather (nvtb_join_gather of the
+(nvtb_mask_count, with its host read), select (nvtb_mask_select), gather (nvtb_gather_rows of the
 fixed-width columns) and list_copy (the list column's offsets gather and nvtb_gb_list_rows).
 Bytes are the algorithmic minimum computed here (every input read once, every output written once,
 row ids read once per gather launch) over the measured time, against 3.35 TB/s (H100 SXM HBM3).
@@ -81,7 +81,7 @@ def _measure(name, frame, make_mask, run_op, steps, warmup, in_bytes):
     out["select"] = _family(_time(lambda: engine.mask_select(mask, n, tile_off, kept), steps, warmup),
                             n / 8 + ntiles * 8 + kept * 8)
     fb = sum(kept * (c.data.element_size() * 2 + (0.25 if c.validity is not None else 0)) for c in flat.values())
-    launches = -(-len(flat) // engine.JOIN_GATHER_MAX_COLS)
+    launches = -(-len(flat) // engine.GATHER_MAX_COLS)
     out["gather"] = _family(_time(lambda: engine.take_rows(flat, rows), steps, warmup), kept * 8 * launches + fb)
     if lists:
         res = engine.take_rows(lists, rows)

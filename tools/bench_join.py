@@ -9,7 +9,8 @@ Two workloads, device-resident:
   expand     1e8 left int32 keys inner-joined to a 1e7-row ext table with about two rows per key
              and 10 % of the left keys missing, carrying int64 and float32 ext columns: probe,
              scan, expand and gather; the key table (16 B slots, 2^24 of them) does not fit in L2
-Prints ONE JSON line: per workload rows/s, output rows/s, per-family CUDA-event times, achieved
+Prints ONE JSON line: per workload rows/s, output rows/s, per-family CUDA-event times (join_probe,
+join_expand, and gather: nvtb_gather_rows of the left and ext columns and list offsets), achieved
 bytes/s of each family against 3.35 TB/s (H100 SXM HBM3) with what bounds it, a parity flag
 against oracle/join_external.py on a seeded 1e5-row sample, and the card name and power limit
 read in the same run.  Writes nothing to the tree."""
@@ -29,7 +30,7 @@ import torch  # noqa: E402
 HBM_BPS = 3.35e12
 BOUNDS = {"join_probe": "one dependent random 16 B table slot per row (latency of L2 / HBM sectors)",
           "join_expand": "two binary searches over the output offsets per 8 output rows",
-          "join_gather": "random ext-row reads at the gathered rows (32 B sectors for 4-8 B values)"}
+          "gather": "random ext-row reads at the gathered rows (32 B sectors for 4-8 B values)"}
 
 
 def _card():
@@ -106,7 +107,7 @@ def _measure(wf, frame, steps, warmup):
     torch.cuda.synchronize()
     fam = {}
     for f, s, e, nbytes in engine.profile:
-        if f.startswith("join_"):
+        if f in BOUNDS:
             ms, b = fam.get(f, (0.0, 0.0))
             fam[f] = (ms + s.elapsed_time(e), b + nbytes)
     engine.profile = None
