@@ -92,7 +92,10 @@ int nvtb_infer_vocab_create(nvtb_infer_vocab_t** out, const int64_t* keys_host, 
   const int64_t mask = cap - 1;
   for (int64_t i = 0; i < n; ++i) {
     const int64_t key = keys_host[i];
-    if (key == nvtb::kEmptyKey) { v->min_key_pos = i; continue; }
+    if (key == nvtb::kEmptyKey) {                      // first wins here too
+      if (v->min_key_pos < 0) v->min_key_pos = i;
+      continue;
+    }
     int64_t s = (int64_t)(nvtb::table_mix64((uint64_t)key) & (uint64_t)mask);
     while (v->slots[2 * s] != nvtb::kEmptyKey && v->slots[2 * s] != key) s = (s + 1) & mask;
     if (v->slots[2 * s] == nvtb::kEmptyKey) { v->slots[2 * s] = key; v->slots[2 * s + 1] = i; }   // first wins

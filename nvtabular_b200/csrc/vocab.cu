@@ -598,7 +598,9 @@ lookup_build_any_kernel(const int64_t* __restrict__ keys, int64_t n, int64_t* sl
                    (int64_t)((uint64_t)table_mix32((uint32_t)(int32_t)k) & (uint64_t)(nbuckets - 1)), nbuckets,
                    ((unsigned long long)(unsigned)(i + 1) << 32) | (unsigned)(int)k);
     } else if (k == kEmptyKey) {
-      *min_key_pos = i;
+      // a repeated key keeps its smallest position, like wide_claim: min of the positions as
+      // unsigned, over the -1 (all ones) the slot starts at
+      atomicMin(reinterpret_cast<unsigned long long*>(min_key_pos), (unsigned long long)i);
     } else {
       wide_claim(slots, capacity, k, (long long)i);
     }
@@ -699,7 +701,6 @@ small_vocab_kernel(const int64_t* __restrict__ keys_in, const int64_t* __restric
     else { slots[2 * i] = kEmptyKey; slots[2 * i + 1] = INT64_MAX; }
   }
   __syncthreads();
-  long long min_pos = -1;
   for (int i = tid; i < n_keep; i += kSmallThreads) {
     const long long key = k[i];
     if (narrow) {                                         // keys are distinct
@@ -708,12 +709,11 @@ small_vocab_kernel(const int64_t* __restrict__ keys_in, const int64_t* __restric
                    (long long)((uint64_t)table_mix32((uint32_t)(int32_t)key) & (uint64_t)(nbuckets - 1)), nbuckets,
                    ((unsigned long long)(unsigned)(i + 1) << 32) | (unsigned)(int)key);
     } else if (key == kEmptyKey) {
-      min_pos = i;
+      atomicMin(reinterpret_cast<unsigned long long*>(&sc->min_key_pos), (unsigned long long)i);   // as lookup_build_any_kernel
     } else {
       wide_claim(slots, capacity, key, i);
     }
   }
-  if (min_pos >= 0) sc->min_key_pos = min_pos;
   if (tid == 0) {
     long long a = 0, b = 0;
     for (int w = 0; w < kSmallThreads / 32; ++w) { a += red[0][w]; b += red[1][w]; }
