@@ -151,6 +151,15 @@ int nvtb_hash_bucket_apply(const nvtb_col_t* cols_host, int ncols, int64_t n,
 int nvtb_hash_values(const nvtb_col_t* col_host, int64_t n, uint64_t* out,
                      void* stream);
 
+/* pack two key columns into one order-preserving int64 key:
+ * (a << 32) | (b ^ 0x80000000), both I32.  Rows where BOTH are null become
+ * null (validity_out bit cleared); a single null becomes INT32_MIN so the
+ * tuple sorts first (categorify.py:1689-1692 all-null rule; KAT
+ * tests/unit/ops/test_categorify.py:288-297). */
+int nvtb_pack_keys2(const nvtb_col_t* a_host, const nvtb_col_t* b_host,
+                    int64_t n, int64_t* keys_out, uint8_t* validity_out,
+                    void* stream);
+
 /* ---- hash aggregation: groupby(key, dropna=False).agg(size[,sum,...]) ----
  * Replaces _top_level_groupby / _mid_level_groupby / _bottom_level_groupby
  * (reference nvtabular/ops/categorify.py:955-1137): cuDF hash-groupby per
@@ -256,32 +265,20 @@ int nvtb_radix_sort_u32(uint32_t* data, uint32_t* tmp, int64_t n, int lo_bit, in
 int nvtb_radix_sort_u64(uint64_t* data, uint64_t* tmp, int64_t n, int lo_bit, int hi_bit,
                         int descending, int* result_in_tmp_host, void* stream);
 
-/* owner = mix(key) % n_parts for the key-hash sharding across GPUs
- * (SURVEY.md §8e; the reference's split_out shuffle_group,
- * categorify.py:1036-1049).  perm_out receives a permutation that groups
- * rows by owner; part_counts_host the rows per owner.  Synchronises. */
-int nvtb_partition_by_owner(const int64_t* keys, int64_t n, int n_parts,
-                            int64_t* perm_out, int64_t* part_counts_host,
-                            void* stream);
-/* same grouping without a host round trip: the per-owner row counts stay on the
- * device (part_counts_dev, int64[n_parts]); nothing synchronises, so the 26
- * columns of a Categorify fit are partitioned back to back and their counts read
- * with ONE copy (nvtabular_b200/dist.py global_merge_many). */
+/* ---- cross-GPU exchange ---- */
+/* owner = mix(key) % n_parts for the key-hash sharding of the hash-table
+ * columns across GPUs (SURVEY.md §8e; the reference's split_out shuffle_group,
+ * categorify.py:1036-1049).  perm_out receives a permutation that groups rows
+ * by owner; part_counts_dev (device int64[n_parts]) the rows per owner.
+ * Nothing synchronises, so the 26 columns of a Categorify fit are partitioned
+ * back to back and their counts read with ONE copy (nvtabular_b200/dist.py
+ * global_merge_many). */
 int nvtb_partition_by_owner_async(const int64_t* keys, int64_t n, int n_parts,
                                   int64_t* perm_out, int64_t* part_counts_dev, void* stream);
 int nvtb_gather_i64(const int64_t* src, const int64_t* perm, int64_t n,
                     int64_t* dst, void* stream);
 int nvtb_gather_f64_rows(const double* src, const int64_t* perm, int64_t n,
                          int row_width, double* dst, void* stream);
-
-/* pack two key columns into one order-preserving int64 key:
- * (a << 32) | (b ^ 0x80000000), both I32.  Rows where BOTH are null become
- * null (validity_out bit cleared); a single null becomes INT32_MIN so the
- * tuple sorts first (categorify.py:1689-1692 all-null rule; KAT
- * tests/unit/ops/test_categorify.py:288-297). */
-int nvtb_pack_keys2(const nvtb_col_t* a_host, const nvtb_col_t* b_host,
-                    int64_t n, int64_t* keys_out, uint8_t* validity_out,
-                    void* stream);
 
 /* ---- vocabulary: ordering, cut, lookup table, encode ----------------------
  * nvtb_vocab_build replaces _write_uniques + _save_encodings (reference

@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libnvtb200.so")
 # the flags the library was built with; a library built with other flags (another architecture)
 # is rebuilt even when it is newer than every source
 FLAGS_STAMP = LIB_PATH + ".flags"
-SOURCES = ["scan_kernels.cu", "hashagg.cu", "sortacc.cu", "vocab.cu", "infer.cu", "comm.cu", "groupby.cu", "artifacts.cu", "join.cu", "session.cu", "filter.cu", "gather.cu"]
+SOURCES = ["scan_kernels.cu", "hashagg.cu", "sortacc.cu", "vocab.cu", "infer.cu", "comm.cu", "groupby.cu", "artifacts.cu", "join.cu", "session.cu", "filter.cu", "gather.cu", "exchange.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
     *GENCODE,

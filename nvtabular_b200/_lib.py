@@ -75,7 +75,6 @@ _SIGNATURES = {
     "nvtb_segment_copy_u64": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_void_p]),
     "nvtb_radix_sort_u32": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, POINTER(c_int), c_void_p]),
     "nvtb_radix_sort_u64": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, POINTER(c_int), c_void_p]),
-    "nvtb_partition_by_owner": (c_int, [c_void_p, c_int64, c_int, c_void_p, POINTER(c_int64), c_void_p]),
     "nvtb_partition_by_owner_async": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
     "nvtb_gather_i64": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "nvtb_gather_f64_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),

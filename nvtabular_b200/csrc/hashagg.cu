@@ -1,5 +1,9 @@
 // hashagg.cu — K3: device hash aggregation  groupby(key, dropna=False).agg(...)
 //
+// The group-by handle's hash table: its layouts, inserts, merges of pre-aggregated rows, the
+// overflow arena and settle, export, and the hand-off of high-cardinality int32 columns to
+// the sorted accumulator (sortacc.cu).
+//
 // Replaces the reference's per-partition cuDF groupby + concat/groupby tree
 // (nvtabular/ops/categorify.py:955-1137, graph built at :1344-1540) with ONE
 // resident open-addressing table per column group that every batch is folded
@@ -691,17 +695,45 @@ rehash_kernel(Table old_t, Table new_t) {
 
 constexpr int kExportPerThread = 4;
 
-// compaction: table -> dense (unordered) arrays.  A CTA compacts 1024 slots at a time and
-// reserves its output range with ONE atomic: a per-warp atomicAdd on the single cursor
-// (500 k same-address atomics for a 16 M-slot table) serialised at ~1 ns each and cost
-// ~20x the time the scan itself needs.
+// A CTA compacts 1024 slots at a time and reserves its output range with ONE atomic: a
+// per-warp atomicAdd on the single cursor (500 k same-address atomics for a 16 M-slot table)
+// serialised at ~1 ns each and cost ~20x the time the scan itself needs.  `mine` = the lane's
+// live slots; returns the lane's first output index.  The caller syncs before reusing
+// s_warp / s_base.
+__device__ __forceinline__ int64_t reserve_range(unsigned mine, unsigned* s_warp, unsigned long long* s_base,
+                                                 unsigned long long* cursor) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned incl = mine;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned y = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += y;
+  }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned tot = 0;
+    for (int w = 0; w < kThreads / 32; ++w) { const unsigned x = s_warp[w]; s_warp[w] = tot; tot += x; }
+    *s_base = tot ? atomicAdd(cursor, (unsigned long long)tot) : 0ull;
+  }
+  __syncthreads();
+  return (int64_t)*s_base + s_warp[warp] + (incl - mine);
+}
+
+// payload {sum, sumsq, min, max} of one group as stored (min / max order-encoded) -> doubles
+__device__ __forceinline__ void decode_payload(const double* v, double* w) {
+  w[0] = v[0]; w[1] = v[1];
+  w[2] = dec_ordered(reinterpret_cast<const int64_t*>(v)[2]);
+  w[3] = dec_ordered(reinterpret_cast<const int64_t*>(v)[3]);
+}
+
+// compaction: table -> dense (unordered) arrays
 __global__ void __launch_bounds__(kThreads)
 export_kernel(Table t, int64_t* __restrict__ keys_out,
               int64_t* __restrict__ sizes_out, double* __restrict__ vals_out,
               unsigned long long* cursor) {
   __shared__ unsigned s_warp[kThreads / 32];
   __shared__ unsigned long long s_base;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   constexpr int64_t kChunk = (int64_t)kThreads * kExportPerThread;
   // capacity is a power of two >= 65536: every chunk is full
   for (int64_t c0 = (int64_t)blockIdx.x * kChunk; c0 < t.capacity; c0 += (int64_t)gridDim.x * kChunk) {
@@ -721,22 +753,7 @@ export_kernel(Table t, int64_t* __restrict__ keys_out,
         if (k[j] != kEmptyKey) { live |= 1u << j; sz[j] = t.slots[2 * s + 1]; }
       }
     }
-    const unsigned mine = __popc(live);
-    unsigned incl = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned y = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += y;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      unsigned tot = 0;
-      for (int w = 0; w < kThreads / 32; ++w) { const unsigned x = s_warp[w]; s_warp[w] = tot; tot += x; }
-      s_base = tot ? atomicAdd(cursor, (unsigned long long)tot) : 0ull;
-    }
-    __syncthreads();
-    int64_t o = (int64_t)s_base + s_warp[warp] + (incl - mine);
+    int64_t o = reserve_range(__popc(live), s_warp, &s_base, cursor);
 #pragma unroll
     for (int j = 0; j < kExportPerThread; ++j) {
       if (!((live >> j) & 1u)) continue;
@@ -744,13 +761,8 @@ export_kernel(Table t, int64_t* __restrict__ keys_out,
       if (sizes_out) sizes_out[o] = sz[j];
       if (vals_out) {
         const int64_t s = c0 + (int64_t)j * kThreads + threadIdx.x;
-        for (int q = 0; q < t.n_agg; ++q) {
-          const double* v = t.vals + (s * t.n_agg + q) * 4;
-          double* w = vals_out + (o * t.n_agg + q) * 4;
-          w[0] = v[0]; w[1] = v[1];
-          w[2] = dec_ordered(reinterpret_cast<const int64_t*>(v)[2]);
-          w[3] = dec_ordered(reinterpret_cast<const int64_t*>(v)[3]);
-        }
+        for (int q = 0; q < t.n_agg; ++q)
+          decode_payload(t.vals + (s * t.n_agg + q) * 4, vals_out + (o * t.n_agg + q) * 4);
       }
       ++o;
     }
@@ -758,13 +770,13 @@ export_kernel(Table t, int64_t* __restrict__ keys_out,
   }
 }
 
-// narrow hash table -> packed pairs (unordered); same per-CTA range reservation as export_kernel
+// narrow hash table -> packed pairs (unordered)
 static __global__ void __launch_bounds__(kThreads)
 table_to_pairs_kernel(Table t, uint64_t* __restrict__ out, unsigned long long* cursor,
                       unsigned long long* max_count) {
   __shared__ unsigned s_warp[kThreads / 32];
   __shared__ unsigned long long s_base;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
   constexpr int64_t kChunk = (int64_t)kThreads * kExportPerThread;
   uint32_t mx = 0;
   for (int64_t c0 = (int64_t)blockIdx.x * kChunk; c0 < t.capacity; c0 += (int64_t)gridDim.x * kChunk) {
@@ -775,22 +787,7 @@ table_to_pairs_kernel(Table t, uint64_t* __restrict__ out, unsigned long long* c
       w[j] = (unsigned long long)t.slots[c0 + (int64_t)j * kThreads + threadIdx.x];
       if (w[j] != 0ull) live |= 1u << j;
     }
-    const unsigned mine = __popc(live);
-    unsigned incl = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned y = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += y;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      unsigned tot = 0;
-      for (int q = 0; q < kThreads / 32; ++q) { const unsigned x = s_warp[q]; s_warp[q] = tot; tot += x; }
-      s_base = tot ? atomicAdd(cursor, (unsigned long long)tot) : 0ull;
-    }
-    __syncthreads();
-    int64_t o = (int64_t)s_base + s_warp[warp] + (incl - mine);
+    int64_t o = reserve_range(__popc(live), s_warp, &s_base, cursor);
 #pragma unroll
     for (int j = 0; j < kExportPerThread; ++j) {
       if (!((live >> j) & 1u)) continue;
@@ -808,124 +805,7 @@ table_to_pairs_kernel(Table t, uint64_t* __restrict__ out, unsigned long long* c
 __global__ void decode_special_kernel(const double* special_vals, int n_agg,
                                       double* out) {
   const int i = threadIdx.x;
-  if (i < 2 * n_agg) {
-    const double* v = special_vals + i * 4;
-    double* w = out + i * 4;
-    w[0] = v[0]; w[1] = v[1];
-    w[2] = dec_ordered(reinterpret_cast<const int64_t*>(v)[2]);
-    w[3] = dec_ordered(reinterpret_cast<const int64_t*>(v)[3]);
-  }
-}
-
-// ---------------------------------------------------------------------------
-// owner partition / gathers / key packing
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ int owner_of(int64_t key, int n_parts) {
-  // bits disjoint from both the global and the smem slot bits
-  return (int)((table_mix64((uint64_t)key) >> 52) % (uint64_t)n_parts);
-}
-
-__global__ void __launch_bounds__(kThreads)
-owner_count_kernel(const int64_t* __restrict__ keys, int64_t n, int n_parts,
-                   unsigned long long* counts) {
-  __shared__ unsigned int sc[64];
-  if (threadIdx.x < 64) sc[threadIdx.x] = 0;
-  __syncthreads();
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    atomicAdd(&sc[owner_of(keys[i], n_parts)], 1u);
-  __syncthreads();
-  if (threadIdx.x < n_parts && sc[threadIdx.x])
-    atomicAdd(&counts[threadIdx.x], (unsigned long long)sc[threadIdx.x]);
-}
-
-// exclusive prefix of the per-owner counts -> write cursors (n_parts <= 64: one thread)
-__global__ void owner_prefix_kernel(const unsigned long long* __restrict__ counts, int n_parts,
-                                    unsigned long long* __restrict__ cursors) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    unsigned long long acc = 0;
-    for (int p = 0; p < n_parts; ++p) { cursors[p] = acc; acc += counts[p]; }
-  }
-}
-
-// scatter pass: each CTA ranks its chunk of rows per owner in shared memory and reserves
-// ONE contiguous range per owner with a single global atomic, instead of one global
-// atomic per row on only `n_parts` addresses (which serialised at ~1 row/ns).
-__global__ void __launch_bounds__(kThreads)
-owner_scatter_kernel(const int64_t* __restrict__ keys, int64_t n, int n_parts,
-                     unsigned long long* cursors, int64_t* __restrict__ perm) {
-  constexpr int kPer = 8;                       // rows per thread per chunk
-  __shared__ unsigned int s_cnt[64];
-  __shared__ unsigned long long s_base[64];
-  const int64_t chunk = (int64_t)kThreads * kPer;
-  const int64_t n_chunks = (n + chunk - 1) / chunk;
-  for (int64_t c = blockIdx.x; c < n_chunks; c += gridDim.x) {
-    if (threadIdx.x < 64) s_cnt[threadIdx.x] = 0u;
-    __syncthreads();
-    int own[kPer];
-    unsigned rank[kPer];
-#pragma unroll
-    for (int j = 0; j < kPer; ++j) {
-      const int64_t i = c * chunk + (int64_t)j * kThreads + threadIdx.x;
-      own[j] = -1;
-      if (i < n) {
-        own[j] = owner_of(keys[i], n_parts);
-        rank[j] = atomicAdd(&s_cnt[own[j]], 1u);
-      }
-    }
-    __syncthreads();
-    if (threadIdx.x < n_parts && s_cnt[threadIdx.x])
-      s_base[threadIdx.x] = atomicAdd(&cursors[threadIdx.x], (unsigned long long)s_cnt[threadIdx.x]);
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < kPer; ++j) {
-      const int64_t i = c * chunk + (int64_t)j * kThreads + threadIdx.x;
-      if (own[j] >= 0) perm[s_base[own[j]] + rank[j]] = i;
-    }
-    __syncthreads();
-  }
-}
-
-__global__ void __launch_bounds__(kThreads)
-gather_i64_kernel(const int64_t* __restrict__ src, const int64_t* __restrict__ perm,
-                  int64_t n, int64_t* __restrict__ dst) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    dst[i] = src[perm[i]];
-}
-
-__global__ void __launch_bounds__(kThreads)
-gather_f64_rows_kernel(const double* __restrict__ src, const int64_t* __restrict__ perm,
-                       int64_t n, int w, double* __restrict__ dst) {
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  const int64_t total = n * w;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
-    const int64_t r = i / w, c = i - r * w;
-    dst[i] = src[perm[r] * w + c];
-  }
-}
-
-__global__ void __launch_bounds__(kThreads)
-pack_keys2_kernel(const int32_t* __restrict__ a, const uint8_t* __restrict__ ma,
-                  const int32_t* __restrict__ b, const uint8_t* __restrict__ mb,
-                  int64_t n, int64_t* __restrict__ out, uint8_t* __restrict__ vout) {
-  // one thread per 8 rows so each thread owns one validity byte
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  const int64_t n8 = (n + 7) / 8;
-  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n8; g += stride) {
-    unsigned vb = 0;
-    for (int k = 0; k < 8; ++k) {
-      const int64_t i = g * 8 + k;
-      if (i >= n) break;
-      const bool va = valid1(ma, i), vb_ = valid1(mb, i);
-      const int32_t x = va ? a[i] : INT32_MIN;
-      const int32_t y = vb_ ? b[i] : INT32_MIN;
-      out[i] = (int64_t)(((uint64_t)(uint32_t)x << 32) |
-                         (uint64_t)((uint32_t)y ^ 0x80000000u));
-      if (va || vb_) vb |= 1u << k;
-    }
-    if (vout) vout[g] = (uint8_t)vb;
-  }
+  if (i < 2 * n_agg) decode_payload(special_vals + i * 4, out + i * 4);
 }
 
 // ---------------------------------------------------------------------------
@@ -1675,85 +1555,6 @@ int nvtb_hashagg_flush(nvtb_hashagg_t* h, void* stream) {
 int nvtb_hashagg_mode(nvtb_hashagg_t* h, int* mode_host) {
   NVTB_REQUIRE(h != nullptr && mode_host != nullptr, "NULL argument");
   *mode_host = h->acc != nullptr ? 1 : 0;
-  return NVTB_OK;
-}
-
-int nvtb_partition_by_owner(const int64_t* keys, int64_t n, int n_parts,
-                            int64_t* perm_out, int64_t* part_counts_host, void* stream) {
-  NVTB_REQUIRE(n >= 0 && n_parts >= 1 && n_parts <= 64, "n_parts must be in [1, 64]");
-  NVTB_REQUIRE(part_counts_host != nullptr, "part_counts_host is NULL");
-  for (int p = 0; p < n_parts; ++p) part_counts_host[p] = 0;
-  if (n == 0) return NVTB_OK;
-  NVTB_REQUIRE(keys != nullptr && perm_out != nullptr, "NULL keys/perm");
-  cudaStream_t st = (cudaStream_t)stream;
-  unsigned long long* d = nullptr;
-  NVTB_CUDA_OK(cudaMallocAsync(&d, sizeof(unsigned long long) * 128, st));
-  NVTB_CUDA_OK(cudaMemsetAsync(d, 0, sizeof(unsigned long long) * 128, st));
-  const int grid = plain_grid(n);
-  owner_count_kernel<<<grid, kThreads, 0, st>>>(keys, n, n_parts, d);
-  NVTB_LAUNCH_OK();
-  unsigned long long hc[64];
-  NVTB_CUDA_OK(cudaMemcpyAsync(hc, d, sizeof(unsigned long long) * n_parts, cudaMemcpyDeviceToHost, st));
-  NVTB_CUDA_OK(cudaStreamSynchronize(st));
-  unsigned long long cur[64], acc = 0;
-  for (int p = 0; p < n_parts; ++p) { cur[p] = acc; acc += hc[p]; part_counts_host[p] = (int64_t)hc[p]; }
-  NVTB_CUDA_OK(cudaMemcpyAsync(d + 64, cur, sizeof(unsigned long long) * n_parts, cudaMemcpyHostToDevice, st));
-  owner_scatter_kernel<<<grid, kThreads, 0, st>>>(keys, n, n_parts, d + 64, perm_out);
-  NVTB_LAUNCH_OK();
-  NVTB_CUDA_OK(cudaStreamSynchronize(st));  // `cur` is a host temporary
-  NVTB_CUDA_OK(cudaFreeAsync(d, st));
-  return NVTB_OK;
-}
-
-int nvtb_partition_by_owner_async(const int64_t* keys, int64_t n, int n_parts,
-                                  int64_t* perm_out, int64_t* part_counts_dev, void* stream) {
-  NVTB_REQUIRE(n >= 0 && n_parts >= 1 && n_parts <= 64, "n_parts must be in [1, 64]");
-  NVTB_REQUIRE(part_counts_dev != nullptr, "part_counts_dev is NULL");
-  cudaStream_t st = (cudaStream_t)stream;
-  NVTB_CUDA_OK(cudaMemsetAsync(part_counts_dev, 0, sizeof(int64_t) * n_parts, st));
-  if (n == 0) return NVTB_OK;
-  NVTB_REQUIRE(keys != nullptr && perm_out != nullptr, "NULL keys/perm");
-  unsigned long long* d = nullptr;     // [64] write cursors
-  NVTB_CUDA_OK(cudaMallocAsync(&d, sizeof(unsigned long long) * 64, st));
-  const int grid = plain_grid(n);
-  owner_count_kernel<<<grid, kThreads, 0, st>>>(keys, n, n_parts, reinterpret_cast<unsigned long long*>(part_counts_dev));
-  NVTB_LAUNCH_OK();
-  owner_prefix_kernel<<<1, 32, 0, st>>>(reinterpret_cast<const unsigned long long*>(part_counts_dev), n_parts, d);
-  NVTB_LAUNCH_OK();
-  owner_scatter_kernel<<<grid, kThreads, 0, st>>>(keys, n, n_parts, d, perm_out);
-  NVTB_LAUNCH_OK();
-  NVTB_CUDA_OK(cudaFreeAsync(d, st));
-  return NVTB_OK;
-}
-
-int nvtb_gather_i64(const int64_t* src, const int64_t* perm, int64_t n, int64_t* dst, void* stream) {
-  NVTB_REQUIRE(n >= 0, "n < 0");
-  if (n == 0) return NVTB_OK;
-  NVTB_REQUIRE(src && perm && dst, "NULL pointer");
-  gather_i64_kernel<<<plain_grid(n), kThreads, 0, (cudaStream_t)stream>>>(src, perm, n, dst);
-  NVTB_LAUNCH_OK();
-  return NVTB_OK;
-}
-
-int nvtb_gather_f64_rows(const double* src, const int64_t* perm, int64_t n, int row_width,
-                         double* dst, void* stream) {
-  NVTB_REQUIRE(n >= 0 && row_width >= 1, "bad n/row_width");
-  if (n == 0) return NVTB_OK;
-  NVTB_REQUIRE(src && perm && dst, "NULL pointer");
-  gather_f64_rows_kernel<<<plain_grid(n * row_width), kThreads, 0, (cudaStream_t)stream>>>(src, perm, n, row_width, dst);
-  NVTB_LAUNCH_OK();
-  return NVTB_OK;
-}
-
-int nvtb_pack_keys2(const nvtb_col_t* a, const nvtb_col_t* b, int64_t n,
-                    int64_t* keys_out, uint8_t* validity_out, void* stream) {
-  NVTB_REQUIRE(a && b && n >= 0, "NULL column or n < 0");
-  NVTB_REQUIRE(a->dtype == NVTB_I32 && b->dtype == NVTB_I32, "pack_keys2 needs int32 columns");
-  if (n == 0) return NVTB_OK;
-  NVTB_REQUIRE(a->data && b->data && keys_out, "NULL data");
-  pack_keys2_kernel<<<plain_grid((n + 7) / 8), kThreads, 0, (cudaStream_t)stream>>>(
-      (const int32_t*)a->data, a->validity, (const int32_t*)b->data, b->validity, n, keys_out, validity_out);
-  NVTB_LAUNCH_OK();
   return NVTB_OK;
 }
 

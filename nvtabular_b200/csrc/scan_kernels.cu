@@ -3,6 +3,7 @@
 //   K2  fused FillMissing + Normalize / NormalizeMinMax (transform)
 //       standalone FillMissing (+ `_filled` indicator)
 //   K6  HashBucket (pandas-compatible value hash % num_buckets)
+//       key images of columns: raw value hashes, two int32 keys packed into one int64
 //
 // Reference behaviour restated (not ported — the reference calls cuDF/pandas):
 //   nvtabular/ops/moments.py:64-116, nvtabular/ops/normalize.py:71-90,150-161,
@@ -428,6 +429,30 @@ hash_values_kernel(HashCols hc, uint64_t* __restrict__ out, int64_t n) {
     out[i] = hash_one(hc, 0, i);
 }
 
+// two int32 key columns -> one order-preserving int64 key (multi-column keys of the group-by)
+__global__ void __launch_bounds__(kThreads)
+pack_keys2_kernel(const int32_t* __restrict__ a, const uint8_t* __restrict__ ma,
+                  const int32_t* __restrict__ b, const uint8_t* __restrict__ mb,
+                  int64_t n, int64_t* __restrict__ out, uint8_t* __restrict__ vout) {
+  // one thread per 8 rows so each thread owns one validity byte
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int64_t n8 = (n + 7) / 8;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n8; g += stride) {
+    unsigned vb = 0;
+    for (int k = 0; k < 8; ++k) {
+      const int64_t i = g * 8 + k;
+      if (i >= n) break;
+      const bool va = valid1(ma, i), vb_ = valid1(mb, i);
+      const int32_t x = va ? a[i] : INT32_MIN;
+      const int32_t y = vb_ ? b[i] : INT32_MIN;
+      out[i] = (int64_t)(((uint64_t)(uint32_t)x << 32) |
+                         (uint64_t)((uint32_t)y ^ 0x80000000u));
+      if (va || vb_) vb |= 1u << k;
+    }
+    if (vout) vout[g] = (uint8_t)vb;
+  }
+}
+
 static int check_cols(const nvtb_col_t* cols, int ncols, int64_t n) {
   NVTB_REQUIRE(ncols >= 0, "ncols < 0");
   NVTB_REQUIRE(n >= 0, "n < 0");
@@ -645,6 +670,18 @@ int nvtb_hash_values(const nvtb_col_t* col, int64_t n, uint64_t* out, void* stre
   memset(&hc, 0, sizeof(hc));
   hc.ncols = 1; hc.data[0] = col->data; hc.mask[0] = col->validity; hc.dtype[0] = col->dtype;
   hash_values_kernel<<<scan_grid(n, 8), kThreads, 0, (cudaStream_t)stream>>>(hc, out, n);
+  NVTB_LAUNCH_OK();
+  return NVTB_OK;
+}
+
+int nvtb_pack_keys2(const nvtb_col_t* a, const nvtb_col_t* b, int64_t n,
+                    int64_t* keys_out, uint8_t* validity_out, void* stream) {
+  NVTB_REQUIRE(a && b && n >= 0, "NULL column or n < 0");
+  NVTB_REQUIRE(a->dtype == NVTB_I32 && b->dtype == NVTB_I32, "pack_keys2 needs int32 columns");
+  if (n == 0) return NVTB_OK;
+  NVTB_REQUIRE(a->data && b->data && keys_out, "NULL data");
+  pack_keys2_kernel<<<plain_grid((n + 7) / 8), kThreads, 0, (cudaStream_t)stream>>>(
+      (const int32_t*)a->data, a->validity, (const int32_t*)b->data, b->validity, n, keys_out, validity_out);
   NVTB_LAUNCH_OK();
   return NVTB_OK;
 }

@@ -134,9 +134,9 @@ def allreduce_sum_i64(t: torch.Tensor) -> torch.Tensor:
     return t
 
 
-def exchange_by_owner(keys, sizes, vals, perm, counts):
-    """all-to-all of rows already grouped by owner (perm/counts from
-    nvtb_partition_by_owner).  Returns the rows this rank owns."""
+def exchange_by_owner(keys, sizes, vals, counts):
+    """all-to-all of rows already grouped by owner (counts from
+    engine.partition_by_owner).  Returns the rows this rank owns."""
     import torch.distributed as dist
     dev = keys.device
     send_counts = torch.tensor(counts, dtype=torch.int64, device=dev)
@@ -151,9 +151,9 @@ def exchange_by_owner(keys, sizes, vals, perm, counts):
                                output_split_sizes=rc, input_split_sizes=list(counts))
         return out
 
-    rk = a2a(keys[perm] if perm is not None else keys)
-    rs = a2a(sizes[perm] if perm is not None else sizes)
-    rv = a2a(vals[perm] if perm is not None else vals) if vals is not None else None
+    rk = a2a(keys)
+    rs = a2a(sizes)
+    rv = a2a(vals) if vals is not None else None
     return rk, rs, rv
 
 
@@ -193,7 +193,7 @@ def global_merge(agg, engine=None):
     if vals is not None:
         width = agg.n_agg * 4
         sv = engine.gather_f64_rows(vals.reshape(-1, width), perm, width)
-    rk, rs, rv = exchange_by_owner(sk, ss, sv, None, counts)
+    rk, rs, rv = exchange_by_owner(sk, ss, sv, counts)
     owner = engine.HashAgg(agg.n_agg, capacity_hint=max(rk.numel(), 1))
     owner.merge(rk, rs, rv.reshape(-1) if rv is not None else None)
     ok, os_, ov, _, _ = owner.export()
@@ -249,18 +249,11 @@ def global_merge_many(aggs, engine=None, owner_pool=None):
     # 1. group every column's rows by owner rank
     # (no host round trip per column: counts stay on the device until all 26 are queued)
     grouped = []
-    if hasattr(engine, "partition_by_owner_async"):
-        counts_dev = torch.zeros((nc, w), dtype=torch.int64, device=dev)
-        for c, (k, s, _, _, _) in enumerate(exported):
-            perm = engine.partition_by_owner_async(k, w, counts_dev[c])
-            grouped.append((engine.gather_i64(k, perm), engine.gather_i64(s, perm)))
-        counts_nc = counts_dev.cpu()
-    else:                                   # stand-in engines of the CPU tests
-        counts_nc = torch.zeros((nc, w), dtype=torch.int64)
-        for c, (k, s, _, _, _) in enumerate(exported):
-            perm, cnt = engine.partition_by_owner(k, w)
-            grouped.append((engine.gather_i64(k, perm), engine.gather_i64(s, perm)))
-            counts_nc[c] = torch.tensor(cnt, dtype=torch.int64)
+    counts_dev = torch.zeros((nc, w), dtype=torch.int64, device=dev)
+    for c, (k, s, _, _, _) in enumerate(exported):
+        perm = engine.partition_by_owner_async(k, w, counts_dev[c])
+        grouped.append((engine.gather_i64(k, perm), engine.gather_i64(s, perm)))
+    counts_nc = counts_dev.cpu()
     send_k = [[None] * nc for _ in range(w)]
     send_s = [[None] * nc for _ in range(w)]
     counts = counts_nc.t().contiguous()     # [owner rank, column]

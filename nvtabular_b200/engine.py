@@ -349,14 +349,11 @@ class HashAgg:
 
 
 def partition_by_owner(keys: torch.Tensor, n_parts: int):
-    """-> (perm int64[n], counts list[int]) grouping rows by hash-owner."""
-    lib = _lib.load()
-    n = keys.numel()
-    perm = torch.empty(n, dtype=torch.int64, device=keys.device)
-    counts = (c_int64 * n_parts)()
-    _lib.check(lib.nvtb_partition_by_owner(_ptr(keys), n, n_parts, _ptr(perm), counts, _lib.stream_ptr()))
-    _count(2)
-    return perm, [int(c) for c in counts]
+    """-> (perm int64[n], counts list[int]) grouping rows by hash-owner; one synchronising
+    read of the counts."""
+    counts = torch.empty(n_parts, dtype=torch.int64, device=keys.device)
+    perm = partition_by_owner_async(keys, n_parts, counts)
+    return perm, counts.tolist()
 
 
 def partition_by_owner_async(keys: torch.Tensor, n_parts: int, counts_out: torch.Tensor):
